@@ -8,7 +8,7 @@ import os
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("MXB_LIB_PATH") or os.path.join(HERE, "lib", "libmaxib200.so")   # override: A/B builds of the same ABI
+LIB_PATH = os.path.join(HERE, "lib", "libmaxib200.so")
 
 MEM_HOST, MEM_DEVICE, MEM_SPLIT, MEM_ASYNC = 0, 1, 2, 0x100
 F64, F32 = 0, 1

@@ -685,7 +685,7 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     if (b->desc.delay_taps > 0) {
         DelayArgs da;
         da.phase = b->dl_phase; da.size = b->dl_size; da.feedback = b->dp[MXB_P_DELAY_FEEDBACK];
-        da.ring = b->ring; da.taps = b->desc.delay_taps; da.W_out = 0;
+        da.ring = b->ring; da.taps = b->desc.delay_taps;
         da.from_position = b->desc.delay_mode == MXB_DELAY_FROM_POSITION ? 1 : 0; da.position = b->dl_pos;
         da.size_tv = d_ds;
         rc = launch_delay_bank(a, da, fk, svf_lp, env, out != nullptr, mix != nullptr, s);

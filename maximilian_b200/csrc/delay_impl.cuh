@@ -37,39 +37,20 @@ namespace mxb {
 constexpr int kDlT = kDlChunk;                    // steps per staged window
 constexpr int kDlRow = kDlT;                      // tile row stride in doubles: unpadded, slot j of row i at position j ^ (i % 16)
 constexpr int kStageDoubles = 32 * kDlRow;        // one staged window tile per warp (4 KB: the image one bulk copy moves)
-// CTA shape of K2. Without a mix tile a warp needs 8 KB of staging: 4 warps per CTA (MXB_DL_THREADS), 24 warps per SM. Left alone,
+// CTA shape of K2. Without a mix tile a warp needs 8 KB of staging: 4 warps per CTA, 24 warps per SM. Left alone,
 // ptxas gives the block-constant kernels 96 registers on sm_90a, which leaves 20 warps per SM; the launch bound holds them to 80
 // (a few bytes of spill) for the 24, which runs ~3 % faster on an H100. With the mix tile (8-row tile: 12.1 KB per warp with the
 // two window stages) shared memory allows 4 CTAs of 4 warps per SM.
-#ifndef MXB_DL_THREADS
-#define MXB_DL_THREADS 128
-#endif
-#ifndef MXB_DL_STAGES
-#define MXB_DL_STAGES 2
-#endif
 template <bool MIX> struct DelayShape {
-    static constexpr int kThreads = MIX ? 128 : MXB_DL_THREADS;
+    static constexpr int kThreads = 128;
     static constexpr int kMinCtas = (MIX ? 16 : 24) * 32 / kThreads;     // resident CTAs per SM the registers must allow
 };
-#ifndef MXB_DL_AHEAD
-#define MXB_DL_AHEAD (MXB_DL_STAGES - 1)
-#endif
-constexpr int kDlStages = MXB_DL_STAGES;          // staged windows per warp
-constexpr int kDlAhead = MXB_DL_AHEAD;            // the bulk path requests this many windows ahead
-// The stage a request refills last held window k + ahead - stages; its write-back was committed kDlSlack groups before the latest one.
-// With slack 0 the warp waits, every window, for the copy engine to have drained the write-back it issued a moment ago (and that
-// drains at the speed of the saturated memory system); with slack 1 the engine has a whole window of time.
-constexpr int kDlSlack = kDlStages - 1 - kDlAhead;
-static_assert(kDlStages >= 2 && kDlStages <= 8 && kDlAhead >= 1 && kDlSlack >= 0 && kDlSlack <= 2, "stages / ahead");
+constexpr int kDlStages = 2;                      // staged windows per warp: window k + 1 is requested while window k is computed
 constexpr int kDlVoicesPerReq = 32 / kDlT;        // voices covered by one cooperative request (2)
 // Rows (steps) of the per-warp mix tile of K2. The tile costs shared memory the window stages compete for: with 16 rows a 4-warp CTA
 // needs 65 KB (3 CTAs = 12 warps per SM), with 8 rows 48.5 KB (4 CTAs = 16 warps per SM) at twice the row-sum instructions -- K2 has
 // the fp64 slots for them, unlike K1. The 8-row tile was the faster of the two for out + mix.
-#ifndef MXB_DL_MIXROWS
-#define MXB_DL_MIXROWS 8
-#endif
-constexpr int kDlMixRows = MXB_DL_MIXROWS;
-static_assert(kDlMixRows == 8 || kDlMixRows == 16, "mix tile rows");
+constexpr int kDlMixRows = 8;
 constexpr int kMixDoubles = 2 * kDlMixRows * 33;
 constexpr int kFastMinSize = 2 * kDlT;
 constexpr unsigned kFull = 0xffffffffu;
@@ -79,10 +60,6 @@ static_assert(kDlT % kDlMixRows == 0, "a staged window is a whole number of mix 
 __device__ __forceinline__ void cp_async8(double* smem_dst, const double* gsrc) {
     const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"(d), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async16(double* smem_dst, const double* gsrc) {
-    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d), "l"(gsrc) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait1() { asm volatile("cp.async.wait_group 1;\n" ::: "memory"); }
@@ -106,11 +83,6 @@ __device__ __forceinline__ void bulk_s2g(void* gdst, const void* smem_src, unsig
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }   // sources read: smem reusable
-template <int PENDING> __device__ __forceinline__ void bulk_wait_read() {      // all but the latest PENDING groups have read their sources
-    if (PENDING == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-    else if (PENDING == 1) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-    else asm volatile("cp.async.bulk.wait_group.read 2;" ::: "memory");
-}
 __device__ __forceinline__ void bulk_wait_but7() { asm volatile("cp.async.bulk.wait_group 7;" ::: "memory"); }         // all but the latest 7 groups performed
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }           // writes performed
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -137,7 +109,7 @@ __device__ __forceinline__ void dl_stage(DlVoice& s, double* row, const int tn, 
                                          const bool relmode, const int swz) {
     double* out64 = (double*)a.out + (size_t)t0 * V + v;
     float* out32 = (float*)a.out + (size_t)t0 * V + v;
-    for (int jb = 0; jb < tn; jb += kDlMixRows) {         // one mix tile (the whole window when the tile has 16 rows)
+    for (int jb = 0; jb < tn; jb += kDlMixRows) {         // one mix tile
     const int jn = min(kDlMixRows, tn - jb);
 #pragma unroll 4
     for (int jj = 0; jj < jn; ++jj) {
@@ -145,8 +117,8 @@ __device__ __forceinline__ void dl_stage(DlVoice& s, double* row, const int tn, 
         const int t = t0 + j;
         if (MODW && a.freq_tv) {
             const bool pb = OSC == OSC_T_GENERIC && a.osc_kind == MXB_OSC_PHASORBETWEEN;
-            if (MXB_FM_PREFETCH > 0 && s.live && t + MXB_FM_PREFETCH < a.n_frames)          // look-ahead on the stream, as in K1
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(a.freq_tv + (size_t)(t + MXB_FM_PREFETCH) * V + v));
+            if (s.live && t + kFmPrefetch < a.n_frames)          // look-ahead on the stream, as in K1
+                asm volatile("prefetch.global.L2 [%0];" ::"l"(a.freq_tv + (size_t)(t + kFmPrefetch) * V + v));
             const double fq = s.live ? a.freq_tv[(size_t)t * V + v] : 1.0;
             s.inc = pb ? ((s.pend - s.duty) / (a.sr / fq)) : osc_increment(a.sr, fq);
         }
@@ -313,83 +285,36 @@ __global__ void __launch_bounds__(DelayShape<MIX>::kThreads, DelayShape<MIX>::kM
         }
         fence_proxy_async();                                                // the initialised barriers become visible to the copy engine
         __syncwarp();
-        // Window k lives in stage k % kDlStages and is requested `ahead` windows early. The windows in flight must be distinct chunks
-        // of the ring (a short ring falls back to one window ahead), and the chunk a request reads must not be the target of a
-        // write-back still under way: the write-back of window k - j hits the chunk of window k + ahead when ahead + j is a multiple
-        // of nchunks, first at j = nchunks - ahead. A ring of at least ahead + 8 chunks only needs the write-backs older than the
-        // latest seven performed (cp.async.bulk.wait_group 7: they were issued seven windows ago, the wait is free); a shorter
-        // ring waits for all of them.
-        const int ahead = nchunks >= kDlStages ? kDlAhead : 1;
-        const bool tight = nchunks - ahead < 8;
+        // Window k lives in stage k % 2 and is requested one window early. The chunk a request reads must not be the target of a
+        // write-back still under way: the write-back of window k - j hits the chunk of window k + 1 when 1 + j is a multiple of
+        // nchunks, first at j = nchunks - 1. A ring of at least 9 chunks only needs the write-backs older than the latest seven
+        // performed (cp.async.bulk.wait_group 7: they were issued seven windows ago, the wait is free); a shorter ring waits for all
+        // of them.
+        const bool tight = nchunks < 9;
         auto chunk_of = [&](int kk) { return (int)(((long long)(base0 >> kDlShift) + kk) % nchunks); };
-#ifdef MXB_DL_NO_TMA
-        static_assert(kDlChunk == 16, "the no-copy-engine A/B path is written for 16-slot windows");
-        // A/B build (scripts/build_variant_one.sh): no copy engine at all -- the window image by 8 coalesced 16-byte cp.async per lane,
-        // cp.async groups for completion.
-        const int nd = nlive * kDlChunk;
-        auto request = [&](double* stage, const double* g) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const int o = 64 * i + 2 * lane;
-                if (o < nd) cp_async16(stage + o, g + o);
-            }
-            cp_async_commit();
-        };
-        for (int j = 0; j < ahead; ++j) {
-            if (j < nstages) request(wsm + j * kStageDoubles, run + (size_t)chunk_of(j) * V * kDlChunk);
-            else cp_async_commit();
+        if (lane == 0 && nstages > 0) {
+            mbar_expect_tx(&bar[0], bytes);
+            bulk_g2s(wsm, run + (size_t)chunk_of(0) * V * kDlChunk, bytes, &bar[0]);
         }
-#else
-        if (lane == 0) {
-            for (int j = 0; j < ahead && j < nstages; ++j) {
-                mbar_expect_tx(&bar[j], bytes);
-                bulk_g2s(wsm + j * kStageDoubles, run + (size_t)chunk_of(j) * V * kDlChunk, bytes, &bar[j]);
-            }
-        }
-#endif
         const int swz = dl_swz((size_t)lane);
-        int sidx = 0, nidx = ahead % kDlStages;                            // stage of window k / of window k + ahead
+        int sidx = 0, nidx = 1;                                             // stage of window k / of window k + 1
         unsigned par = 0;                                                   // parity of stage sidx's barrier: flips every kDlStages windows
-        int nchunk = chunk_of(ahead);
+        int nchunk = chunk_of(1);
         for (int k = 0; k < nstages; ++k) {
             double* buf = wsm + sidx * kStageDoubles;
             const int t0 = k * kDlT;
             const int tn = min(kDlT, a.n_frames - t0);
-#ifdef MXB_DL_NO_TMA
-            if (k + ahead < nstages) request(wsm + nidx * kStageDoubles, run + (size_t)nchunk * V * kDlChunk);
-            else cp_async_commit();                                         // an empty group keeps the count uniform
-            if (ahead == 1) asm volatile("cp.async.wait_group 1;\n" ::: "memory");
-            else asm volatile("cp.async.wait_group %0;\n" ::"n"(kDlAhead) : "memory");
-            __syncwarp();                                                   // every lane's part of window k has landed
-#else
-            if (k + ahead < nstages && lane == 0) {
-                // stage nidx last held window k + ahead - kDlStages (<= k - 1), source of a write-back: wait until the engine has READ it
-                if (tight) bulk_wait_all(); else { if (ahead == kDlAhead) bulk_wait_read<kDlSlack>(); else bulk_wait_read0(); bulk_wait_but7(); }
+            if (k + 1 < nstages && lane == 0) {
+                // stage nidx last held window k - 1, source of a write-back: wait until the engine has READ it
+                if (tight) bulk_wait_all(); else { bulk_wait_read0(); bulk_wait_but7(); }
                 mbar_expect_tx(&bar[nidx], bytes);
                 bulk_g2s(wsm + nidx * kStageDoubles, run + (size_t)nchunk * V * kDlChunk, bytes, &bar[nidx]);
             }
             mbar_wait(&bar[sidx], par);                                     // window k has landed
-#endif
             dl_window<OSC, FILT, ENV, true, OUTMODE, MIX, MODK>(s, buf + lane * kDlChunk, tn, t0, a, d, V, (size_t)vv, lane, gwarp, mixtile, swz);
-#ifdef MXB_DL_NO_TMA
-            // ... and the write-back as a plain coalesced copy of the staged image (8 x 512 B per warp). The buffer is free as soon as
-            // every lane has read its part; every lane later re-reads (cp.async) exactly the bytes it stored: program order is enough.
-            __syncwarp();
-            {
-                double* g = run + (size_t)chunk * V * kDlChunk;
-                const int nd = nlive * kDlChunk;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int o = 64 * i + 2 * lane;
-                    if (o < nd) *(double2*)(g + o) = *(const double2*)(buf + o);
-                }
-            }
-            __syncwarp();
-#else
             fence_proxy_async();                                            // this lane's updates of the window, ordered before the engine reads them
             __syncwarp();
             if (lane == 0) { bulk_s2g(run + (size_t)chunk * V * kDlChunk, buf, bytes); bulk_commit(); }
-#endif
             if (++chunk >= nchunks) chunk = 0;
             if (++nchunk >= nchunks) nchunk = 0;
             if (++sidx == kDlStages) { sidx = 0; par ^= 1u; }
@@ -467,10 +392,10 @@ __global__ void __launch_bounds__(DelayShape<MIX>::kThreads, DelayShape<MIX>::kM
 }
 
 template <int OSC, int FILT, int ENV, int OUTMODE, bool MIX, bool MODK>
-inline int launch_delay_one(const BankArgs& a, const DelayArgs& d, int grid, cudaStream_t s) {
+inline int launch_delay_one(const BankArgs& a, const DelayArgs& d, cudaStream_t s) {
     constexpr int threads = DelayShape<MIX>::kThreads;
     constexpr size_t smem = sizeof(double) * (threads / 32) * (kDlStages * kStageDoubles + (MIX ? kMixDoubles : 0));
-    grid = (a.V + threads - 1) / threads;
+    const int grid = (a.V + threads - 1) / threads;
     auto kern = delay_bank_kernel<OSC, FILT, ENV, OUTMODE, MIX, MODK>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("delay_bank_kernel smem attribute (%zu B): %s", smem, cudaGetErrorString(e)); return MXB_ERR_CUDA; }
@@ -483,14 +408,14 @@ inline int launch_delay_one(const BankArgs& a, const DelayArgs& d, int grid, cud
 // outmode: DL_OUT_*; at least one of outmode / mix is set. MODK: the instantiations for blocks with a per-sample frequency / cutoff
 // (their own translation units, delay_km_*.cu)
 template <int FILT, bool MODK = false>
-inline int launch_delay_filt(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s) {
-#define MXB_D3(O, E)                                                                                       \
-    do {                                                                                                   \
-        if (outmode == DL_OUT_F64)      return mix ? launch_delay_one<O, FILT, E, DL_OUT_F64, true, MODK>(a, d, grid, s)   \
-                                                   : launch_delay_one<O, FILT, E, DL_OUT_F64, false, MODK>(a, d, grid, s); \
-        else if (outmode == DL_OUT_F32) return mix ? launch_delay_one<O, FILT, E, DL_OUT_F32, true, MODK>(a, d, grid, s)   \
-                                                   : launch_delay_one<O, FILT, E, DL_OUT_F32, false, MODK>(a, d, grid, s); \
-        else                            return launch_delay_one<O, FILT, E, DL_OUT_NONE, true, MODK>(a, d, grid, s);       \
+inline int launch_delay_filt(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s) {
+#define MXB_D3(O, E)                                                                                 \
+    do {                                                                                             \
+        if (outmode == DL_OUT_F64)      return mix ? launch_delay_one<O, FILT, E, DL_OUT_F64, true, MODK>(a, d, s)   \
+                                                   : launch_delay_one<O, FILT, E, DL_OUT_F64, false, MODK>(a, d, s); \
+        else if (outmode == DL_OUT_F32) return mix ? launch_delay_one<O, FILT, E, DL_OUT_F32, true, MODK>(a, d, s)   \
+                                                   : launch_delay_one<O, FILT, E, DL_OUT_F32, false, MODK>(a, d, s); \
+        else                            return launch_delay_one<O, FILT, E, DL_OUT_NONE, true, MODK>(a, d, s);       \
     } while (0)
     if (osc_saw) { if (env) MXB_D3(OSC_T_SAW, 1); else MXB_D3(OSC_T_SAW, 0); }
     else         { if (env) MXB_D3(OSC_T_GENERIC, 1); else MXB_D3(OSC_T_GENERIC, 0); }

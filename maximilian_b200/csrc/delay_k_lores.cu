@@ -2,7 +2,7 @@
 #include "delay_impl.cuh"
 
 namespace mxb {
-int launch_delay_lores(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s) {
-    return launch_delay_filt<FILT_T_LORES>(a, d, osc_saw, env, outmode, mix, grid, s);
+int launch_delay_lores(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s) {
+    return launch_delay_filt<FILT_T_LORES>(a, d, osc_saw, env, outmode, mix, s);
 }
 }  // namespace mxb

@@ -5,15 +5,10 @@
 
 namespace mxb {
 
-#ifndef MXB_DL_SHIFT
-#define MXB_DL_SHIFT 4
-#endif
-constexpr int kDlShift = MXB_DL_SHIFT;      // 4, or 3 for an A/B build with 8-slot chunks (half the staging per warp)
+constexpr int kDlShift = 4;
 constexpr int kDlChunk = 1 << kDlShift;     // ring slots per chunk = time steps per staged window (16)
-static_assert(kDlShift == 3 || kDlShift == 4, "chunks of 8 or 16 slots");
-// the swizzle of voice v's chunk: v % 16 for 16-slot chunks; (v / 2) % 8 for 8-slot chunks (rows of 64 bytes: two lanes share a
-// 128-byte bank row, the 8 even lanes of a half-warp must differ in the low half of it and the 8 odd ones in the high half)
-__host__ __device__ inline int dl_swz(size_t v) { return (int)((v >> (4 - kDlShift)) & (size_t)(kDlChunk - 1)); }
+// the swizzle of voice v's chunk: v % 16
+__host__ __device__ inline int dl_swz(size_t v) { return (int)(v & 15); }
 
 // Ring storage is chunk-interleaved and swizzled: slot r of voice v lives at ((r / 16) * V + v) * 16 + ((r % 16) ^ (v % 16)).
 // A voice's 16-slot chunk is 128 contiguous bytes (4 full sectors whatever its phase), and voices whose
@@ -36,28 +31,27 @@ struct DelayArgs {
     int from_position;       // 1: maxiDelayline::dlFromPosition
     const int* position;     // its position argument per voice
     const double* size_tv;   // optional per-sample size argument [n_frames][V] (integral values), else NULL
-    int W_out;               // [out] warps in the launched grid (mix partials stride)
 };
 
-// warps the K2 grid will have for V voices (the caller sizes the mix partials with it)
+// warps the K2 grid will have for V voices (the caller sizes the mix partials with it and passes it as a.W)
 int delay_bank_warps(int V);
 
-int launch_delay_bank(const BankArgs& a, DelayArgs& d, int filt_kind, bool svf_lp, int env, bool out, bool mix,
+int launch_delay_bank(const BankArgs& a, const DelayArgs& d, int filt_kind, bool svf_lp, int env, bool out, bool mix,
                       cudaStream_t s);
 
 // one launcher per filter family (delay_k_*.cu); outmode 0 none / 1 fp64 / 2 fp32
-int launch_delay_none(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_lores(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_hires(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_svf(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_svf_lp(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_biquad(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
+int launch_delay_none(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_lores(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_hires(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_svf(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_svf_lp(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_biquad(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
 // ... and for blocks with a per-sample oscillator frequency / filter cutoff (delay_km_*.cu)
-int launch_delay_none_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_lores_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_hires_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_svf_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_svf_lp_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
-int launch_delay_biquad_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, int grid, cudaStream_t s);
+int launch_delay_none_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_lores_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_hires_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_svf_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_svf_lp_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+int launch_delay_biquad_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
 
 }  // namespace mxb

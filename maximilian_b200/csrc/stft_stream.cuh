@@ -1,6 +1,6 @@
 // K4s: the 1024-point streaming STFT (+ fused MFCC) kernel -- included by spectral.cu.
 //
-// Same arithmetic as stft_kernel<16> (the reference's float radix-2 transform replayed butterfly for butterfly, see the
+// Same arithmetic as stft_kernel (the reference's float radix-2 transform replayed butterfly for butterfly, see the
 // head of spectral.cu), different schedule:
 //
 //   * one warp transforms TWO channels at once, frame f of channel 2k in the low half and of channel 2k+1 in the high
@@ -154,14 +154,11 @@ __device__ __forceinline__ void untangle2(u64& Ri, u64& Ii, u64& R3, u64& I3, co
     }
 }
 
-#ifndef MXB_STREAM_WARPS
-#define MXB_STREAM_WARPS 8
-#endif
-constexpr int kStreamWarps = MXB_STREAM_WARPS;  // warps per CTA = channel pairs in flight per CTA (groups of 4 warps = 8 frames per MFCC batch)
+constexpr int kStreamWarps = 8;        // warps per CTA = channel pairs in flight per CTA (groups of 4 warps = 8 frames per MFCC batch)
 // 2 x 8 warps caps the kernel at 128 registers; on sm_90a that spills a little, yet 2 x 4 warps (no spill) is slower on the full-spectrum
 // instantiation and only slightly faster on the MFCC one (DESIGN.md, K4s)
-constexpr int kStreamCtasPerSm = kStreamWarps <= 8 ? 2 : 1;
-static_assert(kStreamWarps % 4 == 0 && kStreamWarps <= 28, "4-warp groups, two named barriers each");
+constexpr int kStreamCtasPerSm = 2;
+static_assert(kStreamWarps % 4 == 0, "4-warp groups, two named barriers each");
 // named barrier `id` for the 128 threads of a group; literal ids: a register id would reserve all 16 barriers
 __device__ __forceinline__ void group_barrier(const int id) {
     switch (id) {
