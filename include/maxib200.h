@@ -178,6 +178,8 @@ int32_t mxb_bank_set_param(mxb_bank* bank, int32_t id, const double* values, int
  * with the NEXT mxb_bank_process call. From host memory (page-locked; unchanged until that block has started) the copy
  * runs on the bank's own copy stream into the second of two device buffers, overlapping the blocks already enqueued;
  * the next block waits for it on its stream and switches buffers. From device memory it is one copy on `stream`.
+ * Of several calls for the same id before one mxb_bank_process, synchronous (mxb_bank_set_param) or asynchronous, from host or
+ * device memory, the later call wins: that block and the ones after it read the values of the last call.
  * Parameters that need a host pass (cutoff / resonance / gain: coefficient design; holdtime / delay size: integer
  * conversion) fall back to mxb_bank_set_param. The reference passes these values by argument on every sample. */
 int32_t mxb_bank_set_param_async(mxb_bank* bank, int32_t id, const double* values, int32_t mem, void* stream);

@@ -357,14 +357,17 @@ int32_t mxb_bank_set_param_async(mxb_bank* b, int32_t id, const double* values, 
     DeviceGuard g(b->ctx->device);
     const size_t bytes = sizeof(double) * (size_t)b->V;
     if (mem == MXB_MEM_DEVICE) {
-        // the source was produced on `stream`: one stream-ordered device copy into the buffer the next block reads
+        // the source was produced on `stream`: one stream-ordered device copy into the buffer the next block reads. A host
+        // upload still pending for this id is older and is dropped, so that the next block does not switch to its values: its
+        // copy lands in the other buffer, which nothing reads before the next host upload, queued after it on the copy stream.
+        b->dp_pending[id] = false;
         MXB_CUDA(cudaMemcpyAsync(b->dp[id], values, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream_));
         b->set_mask[id] = true;
         return MXB_OK;
     }
     // Host source: the upload goes to the buffer the running / enqueued blocks do NOT read, on the bank's own copy stream,
-    // so it overlaps them; the next mxb_bank_process waits for it (event) and switches over. The buffer being overwritten
-    // was last read two blocks ago: the copy waits for that kernel only.
+    // so it overlaps them; the next mxb_bank_process waits for it (event) and switches over. The copy waits for the event
+    // recorded when the blocks last switched away from that buffer, i.e. for the end of every block that read it.
     if (!b->up_stream) MXB_CUDA(cudaStreamCreateWithFlags(&b->up_stream, cudaStreamNonBlocking));
     if (!b->ev_up[id]) MXB_CUDA(cudaEventCreateWithFlags(&b->ev_up[id], cudaEventDisableTiming));
     const int tgt = 1 - b->dp_cur[id];
@@ -650,6 +653,12 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
 
     for (int id = 0; id < MXB_P_COUNT; ++id) {
         if (!b->dp_pending[id]) continue;                 // an asynchronous host upload for this block: wait for it on the stream, switch over
+        // every block that reads the old buffer is enqueued on `s` before this point: the event marks their end, and the next
+        // upload into the old buffer waits for it
+        const int old = b->dp_cur[id];
+        if (!b->ev_read[id][old]) MXB_CUDA(cudaEventCreateWithFlags(&b->ev_read[id][old], cudaEventDisableTiming));
+        MXB_CUDA(cudaEventRecord(b->ev_read[id][old], s));
+        b->ev_read_set[id][old] = true;
         MXB_CUDA(cudaStreamWaitEvent(s, b->ev_up[id], 0));
         b->dp_cur[id] ^= 1; b->dp[id] = b->dp_buf[id][b->dp_cur[id]]; b->dp_pending[id] = false;
     }
@@ -704,13 +713,6 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
         if (rc != MXB_OK) return rc;
     }
     b->launches += 1;
-    for (int id = 0; id < MXB_P_COUNT; ++id) {            // double-buffered parameters: remember when this block's reads are over
-        if (!b->dp_buf[id][1]) continue;
-        const int c = b->dp_cur[id];
-        if (!b->ev_read[id][c]) MXB_CUDA(cudaEventCreateWithFlags(&b->ev_read[id][c], cudaEventDisableTiming));
-        MXB_CUDA(cudaEventRecord(b->ev_read[id][c], s));
-        b->ev_read_set[id][c] = true;
-    }
     if (mix) {
         const int rows = n_frames * 2;
         const int threads = kMixReduceThreads, blocks = rows;

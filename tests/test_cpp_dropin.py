@@ -11,14 +11,21 @@ from maximilian_b200 import workloads as W
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "cpp", "patch_poly.cpp")
-EXE = os.path.join(ROOT, "tests", "cpp", "patch_poly")
 
 
-def compile_patch(src=SRC, exe=EXE):
+@pytest.fixture(scope="module")
+def bindir(tmp_path_factory):
+    """The compiled patches are build products: they go to a temporary directory, so that the suite also runs from a read-only
+    checkout."""
+    return tmp_path_factory.mktemp("dropin")
+
+
+def compile_patch(bindir, src=SRC):
     # the library is built by __graft_entry__.build() / python -m maximilian_b200.build; a test session only links against it (on the GPU box
     # the object directory does not travel: build.build() there would recompile every kernel, minutes of GPU-box time)
     lib = build.LIB if os.path.exists(build.LIB) else build.build()
     libdir = os.path.dirname(lib)
+    exe = os.path.join(str(bindir), os.path.splitext(os.path.basename(src))[0])
     cmd = ["g++", "-std=c++17", "-O2", "-Wall", "-I", os.path.join(ROOT, "include"), src, "-o", exe,
            "-L", libdir, "-lmaxib200", "-Wl,-rpath," + libdir]
     subprocess.check_call(cmd)
@@ -26,19 +33,18 @@ def compile_patch(src=SRC, exe=EXE):
 
 
 SRC_SPEC = os.path.join(ROOT, "tests", "cpp", "patch_spectral.cpp")
-EXE_SPEC = os.path.join(ROOT, "tests", "cpp", "patch_spectral")
 
 
-def test_spectral_patch_compiles_against_the_dropin_header():
-    exe = compile_patch(SRC_SPEC, EXE_SPEC)
+def test_spectral_patch_compiles_against_the_dropin_header(bindir):
+    exe = compile_patch(bindir, SRC_SPEC)
     r = subprocess.run([exe], capture_output=True, text=True)
     assert r.returncode == 2 and "usage" in r.stderr
 
 
 @pytest.mark.gpu
-def test_spectral_patch_matches_oracle(port, tmp_path):
+def test_spectral_patch_matches_oracle(port, tmp_path, bindir):
     """maxiFFT / maxiMFCC / maxiIFFT of the C++ layer, fed in ragged chunks, against the oracle fed sample by sample."""
-    exe = compile_patch(SRC_SPEC, EXE_SPEC)
+    exe = compile_patch(bindir, SRC_SPEC)
     C, N, bins, hop, nc = 5, 7 * 1024 + 100, 512, 512, 13
     x = W.channel_streams(C, N, seed=44)
     x.tofile(tmp_path / "in.bin")
@@ -73,16 +79,16 @@ def test_spectral_patch_matches_oracle(port, tmp_path):
     assert np.abs(y - oy).max() <= 2e-5 * np.abs(oy).max()
 
 
-def test_patch_compiles_against_the_dropin_header():
-    exe = compile_patch()
+def test_patch_compiles_against_the_dropin_header(bindir):
+    exe = compile_patch(bindir)
     assert os.path.exists(exe)
     r = subprocess.run([exe], capture_output=True, text=True)
     assert r.returncode == 2 and "usage" in r.stderr
 
 
 @pytest.mark.gpu
-def test_patch_through_routing_matches_oracle(port, tmp_path):
-    exe = compile_patch()
+def test_patch_through_routing_matches_oracle(port, tmp_path, bindir):
+    exe = compile_patch(bindir)
     V, B, NB, cap = 300, 256, 3, 512
     p = W.voice_params(V, seed=31, delay_size=cap, ragged_delay=True)
     gates = [W.gate(V, B, 4 * k) for k in range(NB + 1)]
@@ -109,25 +115,24 @@ def test_patch_through_routing_matches_oracle(port, tmp_path):
 
 
 SRC_POLY = os.path.join(ROOT, "tests", "cpp", "patch_polysynth.cpp")
-EXE_POLY = os.path.join(ROOT, "tests", "cpp", "patch_polysynth")
 
 
-def test_polysynth_port_compiles_against_the_dropin_header():
+def test_polysynth_port_compiles_against_the_dropin_header(bindir):
     """cpp/commandline/maximilian_examples/15.polysynth/main.cpp ported to the block-rate classes: same objects, same expressions."""
-    exe = compile_patch(SRC_POLY, EXE_POLY)
+    exe = compile_patch(bindir, SRC_POLY)
     r = subprocess.run([exe], capture_output=True, text=True)
     assert r.returncode == 2 and "usage" in r.stderr
 
 
 @pytest.mark.gpu
-def test_polysynth_port_matches_oracle(port, tmp_path):
+def test_polysynth_port_matches_oracle(port, tmp_path, bindir):
     """The polysynth example (two pulse VCOs summed into a lores VCF, sinebuf LFO on frequency and cutoff, ADSR applied after the filter,
     notes triggered on single samples by a metronome) through the C++ layer -> patch interpreter, against the same graph
     (tests/patch_cases.py) run by the C oracle with the trigger stream the C++ control code produced: 1e-9 relative (lores designs its
     coefficients on every sample: libdevice cos / sqrt / pow)."""
     import golden_checks as G
     import patch_cases as PC
-    exe = compile_patch(SRC_POLY, EXE_POLY)
+    exe = compile_patch(bindir, SRC_POLY)
     g = G.load("tables")
     np.concatenate([g["sine"], g["transition"], [float(g["sine_before"])]]).astype(np.float64).tofile(tmp_path / "tables.bin")
     NB, B, V = 40, 512, 6
@@ -154,21 +159,20 @@ def test_polysynth_port_matches_oracle(port, tmp_path):
 
 
 SRC_FX = os.path.join(ROOT, "tests", "cpp", "patch_featurex.cpp")
-EXE_FX = os.path.join(ROOT, "tests", "cpp", "patch_featurex")
 
 
-def test_per_sample_feature_extractor_compiles_against_the_dropin_header():
-    exe = compile_patch(SRC_FX, EXE_FX)
+def test_per_sample_feature_extractor_compiles_against_the_dropin_header(bindir):
+    exe = compile_patch(bindir, SRC_FX)
     r = subprocess.run([exe], capture_output=True, text=True)
     assert r.returncode == 2 and "usage" in r.stderr
 
 
 @pytest.mark.gpu
-def test_per_sample_feature_extractor_matches_oracle(port, tmp_path):
+def test_per_sample_feature_extractor_matches_oracle(port, tmp_path, bindir):
     """The reference's per-sample idiom (`if (fft.process(x)) {...}`, `y = ifft.process(mags, phases)` every sample; maxiFFTOctaveAnalyzer /
     maxiBark / maxiMFCC on the fired frame) through the C++ layer's scalar signatures, against the oracle: frame schedule exact, magnitudes
     and octave averages / peaks bit-identical, Bark 1e-12, MFCC 1e-9, resynthesis 2e-5 of max (atan2f / cosf / sinf ulps)."""
-    exe = compile_patch(SRC_FX, EXE_FX)
+    exe = compile_patch(bindir, SRC_FX)
     N, bins, hop, nc = 6 * 1024 + 300, 512, 512, 13
     x = W.channel_streams(1, N, seed=45)
     x.tofile(tmp_path / "in.bin")

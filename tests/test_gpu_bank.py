@@ -472,6 +472,35 @@ def test_delay_size_above_capacity_rejected():
         g.set("delay_size", 65.0)
 
 
+@pytest.mark.parametrize("mix", [False, True], ids=["out", "out+mix"])
+@pytest.mark.parametrize("lead", ["none", "1", "16", "17", "last", "size"])
+@pytest.mark.parametrize("size", [32, 48, 64, 112, 128, 144, 160])
+def test_uniform_schedule_ring_sweep(port, size, lead, mix):
+    """K2's uniform schedule (one bulk copy per window each way) on rings of 2 to 10 chunks: how long a window's request waits
+    for older write-backs depends on the chunk count (all of them below 9 chunks, all but the latest seven from 9 on). Every
+    1024-frame block wraps the ring many times. A first block of `lead` frames sets where the next block starts: slot 16
+    (a warp that starts at chunk 1), the last chunk, or exactly `size` (the index goes back to 0 before the next access);
+    lengths 1, 16 and 17 also end in a short window that writes a whole chunk back. 100 voices: the last warp is partial.
+    Four blocks, then one with a per-sample frequency (the modulated kernel); output, bus, ring index and every ring
+    bit-exact against the oracle."""
+    from test_oracle_vs_reference import fm_frequencies
+    V, B, cap = 100, 1024, 160
+    n0 = {"none": 0, "1": 1, "16": 16, "17": 17, "last": size - 16, "size": size}[lead]
+    p = W.voice_params(V, seed=size, delay_size=size)
+    g = gpu_bank(V, osc="saw", delay=True, delay_capacity=cap, max_frames=B)
+    o = port.Bank(V, osc="saw", delay=True, delay_capacity=cap)
+    W.configure_bank(g, "none", p, delay=True); W.configure_bank(o, "none", p, delay=True)
+    blocks = ([(n0, None)] if n0 else []) + [(B, None)] * 4 + [(B, fm_frequencies(V, B, 0))]
+    for i, (n, f) in enumerate(blocks):
+        og, mg = g.process(n, want_mix=mix, freq_tv=f); oo, mo = o.process(n, want_mix=mix, freq_tv=f)
+        _close(og, oo, False, f"block {i} ({n} frames)")
+        if mix:
+            np.testing.assert_allclose(mg, mo, rtol=1e-9, atol=1e-11, err_msg=f"block {i}")
+        assert np.array_equal(g.get("delay_phase"), o.get("delay_phase")), f"block {i}: ring index"
+    for v in range(V):
+        assert np.array_equal(g.ring(v, cap), o.ring(v, cap)), f"ring of voice {v}"
+
+
 def test_fp32_output_storage(port):
     V, B = 512, 256
     p = W.voice_params(V, seed=12)
@@ -480,6 +509,54 @@ def test_fp32_output_storage(port):
     og, _ = g.process(B, out_dtype=np.float32); oo, _ = o.process(B)
     assert og.dtype == np.float32
     assert np.array_equal(og, oo.astype(np.float32))          # state stays fp64; only the stored sample is rounded
+
+
+# (K1 voices, filter, mix) | (K2 voices, ring sizes, mix, per-sample frequency)
+FP32_CASES = {
+    "k1_even": ("k1", 512, "biquad", False), "k1_even_mix": ("k1", 512, "biquad", True),
+    "k1_odd": ("k1", 513, "biquad", False), "k1_odd_mix": ("k1", 513, "svf", True),
+    "k2_uniform": ("k2", 161, "uniform", False), "k2_uniform_mix": ("k2", 161, "uniform", True),
+    "k2_generic_mix": ("k2", 161, "generic", True), "k2_literal": ("k2", 161, "literal", False),
+    "k2_modulated_mix": ("k2", 161, "modulated", True),
+}
+
+
+@pytest.mark.parametrize("case", list(FP32_CASES))
+def test_fp32_output_storage_paths(port, case):
+    """fp32 storage rounds only the stored sample: the output is the oracle's rounded to float32, bit for bit, and the fp64
+    state, rings and bus are those of an identical bank that stores fp64. K1: the paired store (even V), the scalar store
+    (odd V), each with and without the bus. K2: uniform, generic and literal (< 32 slots) rings and the modulated kernel."""
+    from test_oracle_vs_reference import fm_frequencies
+    kern, V, kind, mix = FP32_CASES[case]
+    B, cap = 256, 128
+    k2 = kern == "k2"
+    filt = "svf" if k2 else kind
+    p = W.voice_params(V, seed=12, delay_size=cap, ragged_delay=kind == "generic")
+    if kind == "literal":
+        p["delay_size"] = 1.0 + np.arange(V) % 31
+    kw = dict(osc="saw", filt=filt, env=k2, delay=k2, delay_capacity=cap)
+    g32 = gpu_bank(V, max_frames=B, **kw); g64 = gpu_bank(V, max_frames=B, **kw); o = port.Bank(V, **kw)
+    for b in (g32, g64, o):
+        W.configure_bank(b, filt, p, env=k2, delay=k2)
+    for blk in range(3):
+        on, off = W.gate(V, B, blk) if k2 else (None, None)
+        f = fm_frequencies(V, B, blk) if kind == "modulated" else None
+        o32, m32 = g32.process(B, on, off, want_mix=mix, out_dtype=np.float32, freq_tv=f)
+        o64, m64 = g64.process(B, on, off, want_mix=mix, freq_tv=f)
+        oo, mo = o.process(B, on, off, want_mix=mix, freq_tv=f)
+        assert o32.dtype == np.float32
+        assert np.array_equal(o32, oo.astype(np.float32)), f"blk{blk}: fp32 output is not the oracle's, rounded"
+        assert np.array_equal(o64, oo), f"blk{blk}"
+        if mix:
+            assert np.array_equal(m32, m64), f"blk{blk}: the bus depends on the output's storage type"
+            np.testing.assert_allclose(m32, mo, rtol=1e-9, atol=1e-11)
+    names = ["phase", "osc_output", "filt0", "filt1"] + (["filt2"] if filt == "svf" else [])
+    names += ["env_amplitude", "env_output", "env_holdcount", "env_flags", "delay_phase"] if k2 else []
+    for name in names:
+        assert np.array_equal(g32.get(name), g64.get(name)), name
+    if k2:
+        for v in range(V):
+            assert np.array_equal(g32.ring(v, cap), g64.ring(v, cap)), f"ring of voice {v}"
 
 
 def test_mix_only_and_determinism(port):
@@ -495,6 +572,59 @@ def test_mix_only_and_determinism(port):
     o = port.Bank(V, osc="saw", filt="biquad"); W.configure_bank(o, "biquad", p)
     _, mo = o.process(B, want_out=False, want_mix=True)
     np.testing.assert_allclose(runs[0], mo, rtol=1e-9, atol=1e-10)
+
+
+@pytest.mark.parametrize("chain", ["k1_biquad", "k2_uniform"])
+def test_mix_only_bus_is_the_out_mix_bus(port, chain):
+    """The bus of a mix-only bank is the bus of an identical bank that also writes `out`, bit for bit, and a second mix-only
+    run reproduces it (fixed summation order); within fp64 reassociation of the oracle's bus. K2: uniform 128-slot rings,
+    ADSR notes, a partial last warp."""
+    V, B, NB, cap = 5000, 256, 3, 128
+    k2 = chain.startswith("k2")
+    filt = "none" if k2 else "biquad"
+    p = W.voice_params(V, seed=13, delay_size=cap)
+    kw = dict(osc="saw", filt=filt, env=k2, delay=k2, delay_capacity=cap)
+    gates = [W.gate(V, B, 4 * blk) if k2 else (None, None) for blk in range(NB)]
+    runs = []
+    for want_out in (False, False, True):
+        g = gpu_bank(V, max_frames=B, **kw)
+        W.configure_bank(g, filt, p, env=k2, delay=k2)
+        runs.append([g.process(B, on, off, want_out=want_out, want_mix=True)[1] for on, off in gates])
+    o = port.Bank(V, **kw); W.configure_bank(o, filt, p, env=k2, delay=k2)
+    for blk, (on, off) in enumerate(gates):
+        assert np.array_equal(runs[0][blk], runs[1][blk]), f"blk{blk}: mix-only runs differ"
+        assert np.array_equal(runs[0][blk], runs[2][blk]), f"blk{blk}: mix-only bus != out+mix bus"
+        _, mo = o.process(B, on, off, want_out=False, want_mix=True)
+        np.testing.assert_allclose(runs[0][blk], mo, rtol=1e-9, atol=1e-10)
+
+
+@pytest.mark.parametrize("f32", [False, True], ids=["f64", "f32"])
+def test_misaligned_device_output(port, f32):
+    """K1 picks its store flavour once per block: `out` one element past an aligned address (8 bytes for fp64, 4 for fp32) on an
+    even bank, which would otherwise take the paired stores, must take the scalar ones -- the same bits as an aligned `out`,
+    and nothing written outside it."""
+    import torch
+    V, B = 1024, 200
+    dev = torch.device("cuda", 0)
+    dt = torch.float32 if f32 else torch.float64
+    p = W.voice_params(V, seed=14)
+    banks = [gpu_bank(V, osc="saw", filt="svf", max_frames=B) for _ in range(2)]
+    o = port.Bank(V, osc="saw", filt="svf")
+    for b in banks + [o]:
+        W.configure_bank(b, "svf", p)
+    bufs = [torch.full((B * V + 2,), -7.0, dtype=dt, device=dev) for _ in range(2)]
+    views = [bufs[0][:B * V], bufs[1][1:1 + B * V]]
+    assert views[0].data_ptr() % 16 == 0 and views[1].data_ptr() % 16 == (4 if f32 else 8)
+    for blk in range(2):
+        for b, v in zip(banks, views):
+            b.process_device(B, out_ptr=v.data_ptr(), f32=f32)
+        torch.cuda.synchronize()
+        oo, _ = o.process(B)
+        ref = oo.astype(np.float32) if f32 else oo
+        got = [v.cpu().numpy().reshape(B, V) for v in views]
+        assert np.array_equal(got[0], ref), f"blk{blk}: aligned out differs from the oracle"
+        assert np.array_equal(got[1], got[0]), f"blk{blk}: misaligned out differs from aligned out"
+    assert bufs[1][0].item() == -7.0 and bufs[1][-1].item() == -7.0 and bufs[0][-2:].eq(-7.0).all().item()
 
 
 def _slice_indices(V, n_each=704, mid=640):
