@@ -355,7 +355,7 @@ int32_t mxb_exchange_connect(mxb_exchange* ex, const void* all_handles /* world 
 int32_t mxb_exchange_status(mxb_exchange* ex, int32_t* timed_out_ranks);
 int32_t mxb_exchange_destroy(mxb_exchange* ex);
 int32_t mxb_bank_set_exchange(mxb_bank* bank, mxb_exchange* ex /* NULL detaches */);
-/* ... and a voice patch's bus likewise (the patch's mix-reduce kernel has the same exchange fused in): a sharded polysynth ends every block
+/* ... and a voice patch's bus likewise (banks and patches share one mix-reduce kernel with the exchange fused in): a sharded polysynth ends every block
  * with the global stereo bus on every rank. One exchange serves one bank or patch at a time (its sequence numbers count the blocks). */
 int32_t mxb_patch_set_exchange(mxb_patch* patch, mxb_exchange* ex /* NULL detaches */);
 

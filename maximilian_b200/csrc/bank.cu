@@ -39,11 +39,11 @@ struct mxb_bank {
     double* ring;                            // [V][delay_taps]
     double* partials; size_t partials_len;
     double* mix_dev;                         // [max_frames][2]
-    void* out_stage; size_t out_stage_bytes; // staging for MXB_MEM_HOST out
-    double* fm_stage; size_t fm_stage_bytes; // staging for host-resident per-sample frequencies
-    double* cm_stage; size_t cm_stage_bytes; // ... and cutoffs
-    double* ds_stage; size_t ds_stage_bytes; // ... and delay sizes
-    unsigned char* tv_stage; size_t tv_stage_bytes;   // ... and per-sample triggers
+    unsigned char* out_stage; size_t out_stage_len;   // staging for MXB_MEM_HOST out (bytes: fp64 or fp32)
+    double* fm_stage; size_t fm_stage_len;   // staging for host-resident per-sample frequencies
+    double* cm_stage; size_t cm_stage_len;   // ... and cutoffs
+    double* ds_stage; size_t ds_stage_len;   // ... and delay sizes
+    unsigned char* tv_stage; size_t tv_stage_len;     // ... and per-sample triggers
     int64_t launches;
     mxb_exchange* ex;                        // peer-memory mix exchange (multi-GPU), or NULL
 };
@@ -99,80 +99,6 @@ int redesign(mxb_bank* b) {
     return MXB_OK;
 }
 
-constexpr int kMixReduceThreads = 128;
-
-// Sum of one (frame, channel) row of per-warp partials by one CTA: every thread adds a strided subset in ascending
-// order (two interleaved chains), a fixed xor tree per warp, then the four warp sums in a fixed order -- the
-// summation order never changes between runs. Returned to every thread of warp 0; other warps get 0.
-__device__ __forceinline__ double mix_row_sum(const double* __restrict__ p, const int W, double* sm) {
-    double s0 = 0.0, s1 = 0.0;
-    int w = threadIdx.x;
-    for (; w + kMixReduceThreads < W; w += 2 * kMixReduceThreads) { s0 += p[w]; s1 += p[w + kMixReduceThreads]; }
-    if (w < W) s0 += p[w];
-    double s = s0 + s1;
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
-    __syncthreads();
-    return threadIdx.x < 32 ? (sm[0] + sm[1]) + (sm[2] + sm[3]) : 0.0;
-}
-
-__global__ void __launch_bounds__(kMixReduceThreads) mix_reduce_kernel(const double* __restrict__ partials, double* __restrict__ mix, int rows, int W) {
-    __shared__ double sm[kMixReduceThreads / 32];
-    const int row = blockIdx.x;                       // one CTA per row: rows CTAs keep enough loads in flight for HBM
-    const double s = mix_row_sum(partials + (size_t)row * (size_t)W, W, sm);
-    if (threadIdx.x == 0) mix[row] = s;
-}
-
-__device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p) {
-    unsigned long long v;
-    asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-__device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
-    asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-
-// K3 + K6 in one kernel: every row sum of the local reduction (as mix_reduce_kernel) is PUSHED into this rank's lane
-// of every rank's exchange buffer over NVLink (posted stores); the last CTA to finish publishes the flags, waits on
-// its own (local) flags for every peer and adds the world buses in rank order (protocol: exchange.cu).
-__global__ void __launch_bounds__(kMixReduceThreads) mix_reduce_exchange_kernel(const double* __restrict__ partials, double* __restrict__ mix, int rows, int W, const ExchDev x) {
-    __shared__ double sm[kMixReduceThreads / 32];
-    const int row = blockIdx.x;
-    const double s = mix_row_sum(partials + (size_t)row * (size_t)W, W, sm);
-    if (threadIdx.x < x.world) x.dst_payload[threadIdx.x][row] = s;      // thread r -> rank r's buffer
-    __shared__ bool last;
-    __threadfence_system();                           // this CTA's peer stores are ordered before its ticket
-    __syncthreads();
-    if (threadIdx.x == 0) last = atomicAdd(x.ticket, 1u) == gridDim.x - 1;
-    __syncthreads();
-    if (!last) return;
-    if (threadIdx.x < x.world) {
-        __threadfence_system();                       // cumulative: the other CTAs' stores were ordered before their tickets
-        st_release_sys(x.dst_flag[threadIdx.x], x.seq1);
-        // bounded wait: a peer that died (or never launched this block) costs timeout_ns, not a hung box; the bus is then
-        // incomplete and bit `rank` of *status says whose part is missing (mxb_exchange_status / mxb_bank_process report it)
-        const unsigned long long t0 = globaltimer_ns();
-        unsigned spins = 0;
-        while (ld_acquire_sys(x.src_flags + (size_t)threadIdx.x * (kExchFlagBytes / sizeof(unsigned long long))) < x.seq1) {
-            if ((++spins & 1023u) == 0 && globaltimer_ns() - t0 > x.timeout_ns) { atomicOr(x.status, 1u << threadIdx.x); break; }
-        }
-    }
-    if (threadIdx.x == 0) *x.ticket = 0;
-    __syncthreads();
-    for (int i = threadIdx.x; i < rows; i += blockDim.x) {
-        double s = 0.0;
-        for (int r = 0; r < x.world; ++r)             // rank order on every rank: identical bits everywhere, every run
-            s += __ldcg(x.src_payload + (size_t)r * (size_t)x.stride + i);
-        mix[i] = s;
-    }
-}
-
 // ring slots [0, n) of one voice <-> a linear array (set != 0: linear -> ring)
 __global__ void ring_linear_kernel(double* __restrict__ ring, size_t V, size_t voice, double* __restrict__ lin, int n, int set) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
@@ -222,22 +148,7 @@ int32_t mxb_bank_create(mxb_ctx* ctx, const mxb_bank_desc* d, mxb_bank** out) {
     MXB_REQUIRE(g.ok, MXB_ERR_CUDA, "mxb_bank_create: cudaSetDevice failed");
     mxb_bank* b = new (std::nothrow) mxb_bank();
     MXB_REQUIRE(b, MXB_ERR_ALLOC, "mxb_bank_create: out of host memory");
-    b->ctx = ctx; b->desc = *d; b->V = d->voices;
-    for (int i = 0; i < MXB_P_COUNT; ++i) {
-        b->dp[i] = b->dp_buf[i][0] = b->dp_buf[i][1] = nullptr; b->dp_cur[i] = 0; b->dp_pending[i] = false;
-        b->ev_up[i] = nullptr; b->ev_read[i][0] = b->ev_read[i][1] = nullptr; b->ev_read_set[i][0] = b->ev_read_set[i][1] = false;
-    }
-    b->up_stream = nullptr; b->ex = nullptr;
-    b->osc_out = b->f0 = b->f1 = b->f2 = nullptr;
-    for (auto& c : b->cf) c = nullptr;
-    b->env_amp = b->env_output = nullptr; b->env_holdcount = b->env_hold = nullptr; b->env_flags = nullptr;
-    b->trig_on = b->trig_off = b->dl_phase = b->dl_size = b->dl_pos = nullptr;
-    b->ring = b->partials = b->mix_dev = nullptr; b->partials_len = 0;
-    b->out_stage = nullptr; b->out_stage_bytes = 0; b->launches = 0;
-    b->fm_stage = nullptr; b->fm_stage_bytes = 0;
-    b->cm_stage = nullptr; b->cm_stage_bytes = 0;
-    b->ds_stage = nullptr; b->ds_stage_bytes = 0;
-    b->tv_stage = nullptr; b->tv_stage_bytes = 0;
+    b->ctx = ctx; b->desc = *d; b->V = d->voices;           // every other member is value-initialised: zero / NULL
     const size_t V = (size_t)d->voices;
     int rc = MXB_OK;
 #define TRY(x) do { rc = (x); if (rc != MXB_OK) { free_bank(b); return rc; } } while (0)
@@ -290,7 +201,8 @@ int32_t mxb_bank_voices(const mxb_bank* b) { return b ? b->V : MXB_ERR_INVALID; 
 
 int32_t mxb_bank_set_exchange(mxb_bank* b, mxb_exchange* ex) {
     MXB_REQUIRE(b, MXB_ERR_INVALID, "mxb_bank_set_exchange: NULL bank");
-    if (ex) MXB_REQUIRE(ex->ctx->device == b->ctx->device, MXB_ERR_INVALID, "mxb_bank_set_exchange: exchange and bank live on different devices");
+    const int rc = mix_bus_attach(ex, b->ctx->device, "mxb_bank_set_exchange");
+    if (rc != MXB_OK) return rc;
     b->ex = ex;
     return MXB_OK;
 }
@@ -565,9 +477,9 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     if (fk == MXB_FILT_LORES || fk == MXB_FILT_HIRES)
         MXB_REQUIRE(b->set_mask[MXB_P_CUTOFF] && b->set_mask[MXB_P_RESONANCE], MXB_ERR_STATE,
                     "mxb_bank_process: lores/hires need MXB_P_CUTOFF and MXB_P_RESONANCE (they are call arguments in the reference)");
-    if (mix && b->ex) {     // before any kernel runs: a refused call must leave phase / filter / envelope / ring state untouched
-        MXB_REQUIRE(b->ex->connected, MXB_ERR_STATE, "mxb_bank_process: the attached exchange is not connected to its peers");
-        MXB_REQUIRE(n_frames * 2 <= b->ex->max_doubles, MXB_ERR_INVALID, "mxb_bank_process: exchange holds %d values, the bus needs %d", b->ex->max_doubles, n_frames * 2);
+    if (mix) {     // before any kernel runs: a refused call must leave phase / filter / envelope / ring state untouched
+        const int rc = mix_bus_admit(b->ex, n_frames, "mxb_bank_process");
+        if (rc != MXB_OK) return rc;
     }
     if (n_frames == 0) return MXB_OK;
     DeviceGuard g(b->ctx->device);
@@ -583,39 +495,23 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     if (dsize_tv)
         MXB_REQUIRE(b->desc.delay_taps > 0, MXB_ERR_UNSUPPORTED, "mxb_bank_process_mod: delay_size_tv on a bank without a delay line");
     // per-sample parameters are control data: they live where the gates live
-    auto stage = [&](const double* src, double** buf, size_t* cap, const double** dev) -> int {
+    const size_t nv = (size_t)n_frames * V;
+    auto stage = [&](const auto* src, auto** buf, size_t* len, const auto** dev) -> int {
         *dev = src;
         if (!src || !host_ctl) return MXB_OK;
-        const size_t need = sizeof(double) * (size_t)n_frames * V;
-        if (need > *cap) {
-            MXB_CUDA(cudaStreamSynchronize(s));
-            cudaFree(*buf); *buf = nullptr; *cap = 0;
-            cudaError_t e = cudaMalloc((void**)buf, need);
-            if (e != cudaSuccess) { set_error("mxb_bank_process_mod: staging cudaMalloc(%zu): %s", need, cudaGetErrorString(e)); return MXB_ERR_ALLOC; }
-            *cap = need;
-        }
-        MXB_CUDA(cudaMemcpyAsync(*buf, src, need, cudaMemcpyHostToDevice, s));
+        const int rc = ensure(buf, len, nv, s);
+        if (rc != MXB_OK) return rc;
+        MXB_CUDA(cudaMemcpyAsync(*buf, src, sizeof(*src) * nv, cudaMemcpyHostToDevice, s));
         *dev = *buf;
         return MXB_OK;
     };
-    const double *d_fm = nullptr, *d_cm = nullptr;
-    { int rc0 = stage(freq_tv, &b->fm_stage, &b->fm_stage_bytes, &d_fm); if (rc0 != MXB_OK) return rc0; }
-    { int rc0 = stage(cutoff_tv, &b->cm_stage, &b->cm_stage_bytes, &d_cm); if (rc0 != MXB_OK) return rc0; }
-    const double* d_ds = nullptr;
-    { int rc0 = stage(dsize_tv, &b->ds_stage, &b->ds_stage_bytes, &d_ds); if (rc0 != MXB_OK) return rc0; }
-    const unsigned char* d_tv = trig_tv;
-    if (trig_tv && host_ctl) {
-        const size_t need = (size_t)n_frames * V;
-        if (need > b->tv_stage_bytes) {
-            MXB_CUDA(cudaStreamSynchronize(s));
-            cudaFree(b->tv_stage); b->tv_stage = nullptr; b->tv_stage_bytes = 0;
-            cudaError_t e = cudaMalloc((void**)&b->tv_stage, need);
-            if (e != cudaSuccess) { set_error("mxb_bank_process_mod: staging cudaMalloc(%zu): %s", need, cudaGetErrorString(e)); return MXB_ERR_ALLOC; }
-            b->tv_stage_bytes = need;
-        }
-        MXB_CUDA(cudaMemcpyAsync(b->tv_stage, trig_tv, need, cudaMemcpyHostToDevice, s));
-        d_tv = b->tv_stage;
-    }
+    const double *d_fm, *d_cm, *d_ds;
+    const unsigned char* d_tv;
+    int rc = stage(freq_tv, &b->fm_stage, &b->fm_stage_len, &d_fm);
+    if (rc == MXB_OK) rc = stage(cutoff_tv, &b->cm_stage, &b->cm_stage_len, &d_cm);
+    if (rc == MXB_OK) rc = stage(dsize_tv, &b->ds_stage, &b->ds_stage_len, &d_ds);
+    if (rc == MXB_OK) rc = stage(trig_tv, &b->tv_stage, &b->tv_stage_len, &d_tv);
+    if (rc != MXB_OK) return rc;
     if (host_ctl) {
         if (trig_on) {
             MXB_CUDA(cudaMemcpyAsync(b->trig_on, trig_on, sizeof(int) * V, cudaMemcpyHostToDevice, s));
@@ -623,14 +519,8 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
             d_on = b->trig_on; d_off = b->trig_off;
         }
         if (out && host_out) {
-            const size_t need = (size_t)n_frames * V * esz;
-            if (need > b->out_stage_bytes) {
-                MXB_CUDA(cudaStreamSynchronize(s));
-                cudaFree(b->out_stage); b->out_stage = nullptr; b->out_stage_bytes = 0;
-                cudaError_t e = cudaMalloc(&b->out_stage, need);
-                if (e != cudaSuccess) { set_error("mxb_bank_process: staging cudaMalloc(%zu): %s", need, cudaGetErrorString(e)); return MXB_ERR_ALLOC; }
-                b->out_stage_bytes = need;
-            }
+            rc = ensure(&b->out_stage, &b->out_stage_len, nv * esz, s);
+            if (rc != MXB_OK) return rc;
             d_out = b->out_stage;
         }
         if (mix) d_mix = b->mix_dev;
@@ -641,14 +531,8 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     // warps that own at least one voice (warps past the end of the bank exit without writing partials)
     const int W = b->desc.delay_taps > 0 ? delay_bank_warps(b->V) : (int)((V + 32 * kBankVPT - 1) / (32 * kBankVPT));
     if (mix) {
-        const size_t need = (size_t)b->desc.max_frames * 2 * (size_t)W;
-        if (need > b->partials_len) {
-            MXB_CUDA(cudaStreamSynchronize(s));
-            cudaFree(b->partials); b->partials = nullptr; b->partials_len = 0;
-            int rc = dev_alloc(&b->partials, need, false);
-            if (rc != MXB_OK) return rc;
-            b->partials_len = need;
-        }
+        rc = ensure(&b->partials, &b->partials_len, (size_t)b->desc.max_frames * 2 * (size_t)W, s);
+        if (rc != MXB_OK) return rc;
     }
 
     for (int id = 0; id < MXB_P_COUNT; ++id) {
@@ -690,7 +574,6 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     const bool svf_lp = fk == MXB_FILT_SVF && b->desc.svf_mix[0] == 1.0 && b->desc.svf_mix[1] == 0.0 &&
                         b->desc.svf_mix[2] == 0.0 && b->desc.svf_mix[3] == 0.0;
 
-    int rc;
     if (b->desc.delay_taps > 0) {
         DelayArgs da;
         da.phase = b->dl_phase; da.size = b->dl_size; da.feedback = b->dp[MXB_P_DELAY_FEEDBACK];
@@ -714,14 +597,8 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     }
     b->launches += 1;
     if (mix) {
-        const int rows = n_frames * 2;
-        const int threads = kMixReduceThreads, blocks = rows;
-        if (b->ex) {
-            mix_reduce_exchange_kernel<<<blocks, threads, 0, s>>>(b->partials, d_mix, rows, a.W, exchange_next(b->ex));
-        } else {
-            mix_reduce_kernel<<<blocks, threads, 0, s>>>(b->partials, d_mix, rows, a.W);
-        }
-        MXB_CUDA(cudaGetLastError());
+        rc = mix_bus_reduce(b->ex, b->partials, W, n_frames, d_mix, s);
+        if (rc != MXB_OK) return rc;
         b->launches += 1;
     }
     if (host_ctl) {
@@ -729,11 +606,7 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
         if (mix) MXB_CUDA(cudaMemcpyAsync(mix, d_mix, sizeof(double) * (size_t)n_frames * 2, cudaMemcpyDeviceToHost, s));
         if (async_host) return MXB_OK;            // results are valid once `stream` (or the context) has been synchronised
         MXB_CUDA(cudaStreamSynchronize(s));
-        if (mix && b->ex) {       // the call is synchronous in this mode: a timed-out exchange is an error of THIS call
-            unsigned int m = 0;
-            MXB_CUDA(cudaMemcpy(&m, b->ex->status, sizeof(m), cudaMemcpyDeviceToHost));
-            MXB_REQUIRE(m == 0, MXB_ERR_STATE, "mxb_bank_process: mix exchange timed out waiting for rank mask 0x%x (bus incomplete)", m);
-        }
+        if (mix) return mix_bus_status(b->ex, "mxb_bank_process");      // the call is synchronous in this mode: a timed-out exchange is an error of THIS call
     }
     return MXB_OK;
 }

@@ -68,6 +68,18 @@ inline int dev_alloc(T** p, size_t n, bool zero = true) {
     return MXB_OK;
 }
 
+// Grows a staging buffer to at least `need` elements (contents not kept). Work queued on `s` may still read the old
+// buffer, so `s` is synchronised before it is freed.
+template <class T>
+inline int ensure(T** p, size_t* len, size_t need, cudaStream_t s) {
+    if (need <= *len) return MXB_OK;
+    MXB_CUDA(cudaStreamSynchronize(s));
+    cudaFree(*p); *p = nullptr; *len = 0;
+    const int rc = dev_alloc(p, need, false);
+    if (rc == MXB_OK) *len = need;
+    return rc;
+}
+
 }  // namespace mxb
 
 struct mxb_ctx {

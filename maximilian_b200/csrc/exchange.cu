@@ -1,4 +1,5 @@
-// mxb_exchange: symmetric peer-memory buffers for the mix-bus all-reduce (see exchange.cuh, bank.cu).
+// The mix bus (see exchange.cuh): the kernels that reduce the per-warp mix partials of a bank or a voice patch, and
+// mxb_exchange, symmetric peer-memory buffers for the all-reduce of the bus between GPUs.
 //
 // Protocol (per call, sequence number s, slot = s & 1; every rank owns flags[world] + payload[2 slots][world][n], all
 // peer-mapped with CUDA IPC). PUSH model -- nothing is ever read over NVLink, nobody polls remote memory:
@@ -9,7 +10,7 @@
 //      the world buses, all in local HBM, IN RANK ORDER -- every rank computes the same sum, bit for bit, every run
 //   3. slot reuse at call s + 2 is safe: a rank finishes call s + 1 only after every peer's flag reached s + 2, i.e.
 //      after every peer had launched call s + 1 and therefore finished reading slot(s) (stream order on the peer)
-// One kernel does the local reduction and the exchange (bank.cu: mix_reduce_exchange_kernel); nothing here calls NCCL.
+// One kernel does the local reduction and the exchange (mix_reduce_exchange_kernel); nothing here calls NCCL.
 #include <new>
 
 #include "exchange.cuh"
@@ -17,6 +18,116 @@
 using namespace mxb;
 
 namespace mxb {
+
+constexpr int kExchMaxWorld = 16;
+constexpr int kExchFlagBytes = 128;          // one flag per source rank, each alone in its line
+
+// Every rank owns one buffer: flags[kExchMaxWorld] (128 B apart), then payload[2 slots][world][max_doubles].
+// flags[r] / payload[slot][r] are WRITTEN BY RANK r (pushed over NVLink) and read only by the owner, locally.
+struct ExchDev {                              // passed to the kernel by value
+    double* dst_payload[kExchMaxWorld];       // [r]: payload[slot][my rank] inside rank r's buffer (own entry = local)
+    unsigned long long* dst_flag[kExchMaxWorld];   // [r]: flags[my rank] inside rank r's buffer
+    const double* src_payload;                // my buffer: payload[slot][0]
+    const unsigned long long* src_flags;      // my buffer: flags[0]
+    int rank, world, stride;                  // stride = max_doubles (doubles between two source ranks' payloads)
+    unsigned long long seq1;                  // value the flags reach when this call's payload is published
+    unsigned int* ticket;                     // last-CTA election
+    unsigned int* status;                     // bit r set: rank r's flag did not arrive within timeout_ns (sticky)
+    unsigned long long timeout_ns;            // bound of the flag wait
+};
+
+}  // namespace mxb
+
+struct mxb_exchange {
+    mxb_ctx* ctx;
+    int rank, world, max_doubles;
+    size_t flags_bytes, slot_bytes;           // slot = world * max_doubles doubles, 128-byte multiple
+    unsigned char* local;                     // cudaMalloc'ed: flags + 2 slots
+    unsigned char* peers[mxb::kExchMaxWorld]; // cudaIpcOpenMemHandle'd (own entry = local)
+    bool connected;
+    unsigned long long seq;                   // calls so far
+    unsigned int* ticket;
+    unsigned int* status;                     // device word, see ExchDev::status
+    unsigned long long timeout_ns;            // default 5 s; MXB_EXCHANGE_TIMEOUT_MS overrides
+};
+
+namespace {
+
+constexpr int kMixReduceThreads = 128;
+
+// Sum of one (frame, channel) row of per-warp partials by one CTA: every thread adds a strided subset in ascending
+// order (two interleaved chains), a fixed xor tree per warp, then the four warp sums in a fixed order -- the
+// summation order never changes between runs. Returned to every thread of warp 0; other warps get 0.
+__device__ __forceinline__ double mix_row_sum(const double* __restrict__ p, const int W, double* sm) {
+    double s0 = 0.0, s1 = 0.0;
+    int w = threadIdx.x;
+    for (; w + kMixReduceThreads < W; w += 2 * kMixReduceThreads) { s0 += p[w]; s1 += p[w + kMixReduceThreads]; }
+    if (w < W) s0 += p[w];
+    double s = s0 + s1;
+#pragma unroll
+    for (int m = 16; m >= 1; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
+    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
+    __syncthreads();
+    return threadIdx.x < 32 ? (sm[0] + sm[1]) + (sm[2] + sm[3]) : 0.0;
+}
+
+__global__ void __launch_bounds__(kMixReduceThreads) mix_reduce_kernel(const double* __restrict__ partials, double* __restrict__ mix, int rows, int W) {
+    __shared__ double sm[kMixReduceThreads / 32];
+    const int row = blockIdx.x;                       // one CTA per row: rows CTAs keep enough loads in flight for HBM
+    const double s = mix_row_sum(partials + (size_t)row * (size_t)W, W, sm);
+    if (threadIdx.x == 0) mix[row] = s;
+}
+
+__device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p) {
+    unsigned long long v;
+    asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+__device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
+    asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+// K3 + K6 in one kernel: every row sum of the local reduction (as mix_reduce_kernel) is PUSHED into this rank's lane
+// of every rank's exchange buffer over NVLink (posted stores); the last CTA to finish publishes the flags, waits on
+// its own (local) flags for every peer and adds the world buses in rank order (protocol: top of this file).
+__global__ void __launch_bounds__(kMixReduceThreads) mix_reduce_exchange_kernel(const double* __restrict__ partials, double* __restrict__ mix, int rows, int W, const ExchDev x) {
+    __shared__ double sm[kMixReduceThreads / 32];
+    const int row = blockIdx.x;
+    const double s = mix_row_sum(partials + (size_t)row * (size_t)W, W, sm);
+    if (threadIdx.x < x.world) x.dst_payload[threadIdx.x][row] = s;      // thread r -> rank r's buffer
+    __shared__ bool last;
+    __threadfence_system();                           // this CTA's peer stores are ordered before its ticket
+    __syncthreads();
+    if (threadIdx.x == 0) last = atomicAdd(x.ticket, 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!last) return;
+    if (threadIdx.x < x.world) {
+        __threadfence_system();                       // cumulative: the other CTAs' stores were ordered before their tickets
+        st_release_sys(x.dst_flag[threadIdx.x], x.seq1);
+        // bounded wait: a peer that died (or never launched this block) costs timeout_ns, not a hung box; the bus is then
+        // incomplete and bit `rank` of *status says whose part is missing (mxb_exchange_status / mix_bus_status report it)
+        const unsigned long long t0 = globaltimer_ns();
+        unsigned spins = 0;
+        while (ld_acquire_sys(x.src_flags + (size_t)threadIdx.x * (kExchFlagBytes / sizeof(unsigned long long))) < x.seq1) {
+            if ((++spins & 1023u) == 0 && globaltimer_ns() - t0 > x.timeout_ns) { atomicOr(x.status, 1u << threadIdx.x); break; }
+        }
+    }
+    if (threadIdx.x == 0) *x.ticket = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < rows; i += blockDim.x) {
+        double s = 0.0;
+        for (int r = 0; r < x.world; ++r)             // rank order on every rank: identical bits everywhere, every run
+            s += __ldcg(x.src_payload + (size_t)r * (size_t)x.stride + i);
+        mix[i] = s;
+    }
+}
+
+// fills the device descriptor for the next call and advances the sequence
 ExchDev exchange_next(mxb_exchange* ex) {
     ExchDev d;
     memset(&d, 0, sizeof(d));
@@ -31,6 +142,40 @@ ExchDev exchange_next(mxb_exchange* ex) {
     ex->seq += 1;
     return d;
 }
+
+}  // namespace
+
+namespace mxb {
+
+int mix_bus_attach(const mxb_exchange* ex, int device, const char* who) {
+    if (ex) MXB_REQUIRE(ex->ctx->device == device, MXB_ERR_INVALID, "%s: the exchange lives on device %d, the caller on device %d", who, ex->ctx->device, device);
+    return MXB_OK;
+}
+
+int mix_bus_admit(const mxb_exchange* ex, int n_frames, const char* who) {
+    if (!ex) return MXB_OK;
+    MXB_REQUIRE(ex->connected, MXB_ERR_STATE, "%s: the attached exchange is not connected to its peers", who);
+    MXB_REQUIRE(n_frames * 2 <= ex->max_doubles, MXB_ERR_INVALID, "%s: exchange holds %d values, the bus needs %d", who, ex->max_doubles, n_frames * 2);
+    return MXB_OK;
+}
+
+int mix_bus_reduce(mxb_exchange* ex, const double* partials, int W, int n_frames, double* mix, cudaStream_t s) {
+    const int rows = n_frames * 2;      // one CTA per (frame, channel) row
+    if (ex) mix_reduce_exchange_kernel<<<rows, kMixReduceThreads, 0, s>>>(partials, mix, rows, W, exchange_next(ex));
+    else mix_reduce_kernel<<<rows, kMixReduceThreads, 0, s>>>(partials, mix, rows, W);
+    MXB_CUDA(cudaGetLastError());
+    return MXB_OK;
+}
+
+int mix_bus_status(mxb_exchange* ex, const char* who) {
+    if (!ex) return MXB_OK;
+    int32_t m = 0;
+    const int rc = mxb_exchange_status(ex, &m);
+    if (rc != MXB_OK) return rc;
+    MXB_REQUIRE(m == 0, MXB_ERR_STATE, "%s: mix exchange timed out waiting for rank mask 0x%x (bus incomplete)", who, (unsigned)m);
+    return MXB_OK;
+}
+
 }  // namespace mxb
 
 extern "C" {

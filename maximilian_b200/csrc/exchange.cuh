@@ -1,44 +1,21 @@
-// K6: mix-bus exchange between the GPUs of one box over peer memory (NVLink / NVSwitch), fused into the kernel
-// that reduces the per-warp mix partials -- the path's only inter-GPU step (16 KiB per block and rank).
+// The mix bus of a voice bank or a voice patch (K3 + K6): one fixed-order reduction of the per-warp mix partials, with
+// the exchange of the bus between the GPUs of one box over peer memory (NVLink / NVSwitch) fused in when an mxb_exchange
+// is attached -- the path's only inter-GPU step (16 KiB per block and rank). The exchange's buffers and protocol are
+// private to exchange.cu. Every function accepts ex == NULL (no exchange) and starts its error messages with `who`.
 #pragma once
 
 #include "common.cuh"
 
 namespace mxb {
 
-constexpr int kExchMaxWorld = 16;
-constexpr int kExchFlagBytes = 128;          // one flag per source rank, each alone in its line
-
-// Every rank owns one buffer: flags[kExchMaxWorld] (128 B apart), then payload[2 slots][world][max_doubles].
-// flags[r] / payload[slot][r] are WRITTEN BY RANK r (pushed over NVLink) and read only by the owner, locally.
-struct ExchDev {                              // passed to the kernel by value
-    double* dst_payload[kExchMaxWorld];       // [r]: payload[slot][my rank] inside rank r's buffer (own entry = local)
-    unsigned long long* dst_flag[kExchMaxWorld];   // [r]: flags[my rank] inside rank r's buffer
-    const double* src_payload;                // my buffer: payload[slot][0]
-    const unsigned long long* src_flags;      // my buffer: flags[0]
-    int rank, world, stride;                  // stride = max_doubles (doubles between two source ranks' payloads)
-    unsigned long long seq1;                  // value the flags reach when this call's payload is published
-    unsigned int* ticket;                     // last-CTA election
-    unsigned int* status;                     // bit r set: rank r's flag did not arrive within timeout_ns (sticky)
-    unsigned long long timeout_ns;            // bound of the flag wait
-};
+// mxb_{bank,patch}_set_exchange: the exchange must live on the caller's device
+int mix_bus_attach(const mxb_exchange* ex, int device, const char* who);
+// before any kernel of a block runs: the exchange is connected to its peers and holds the block's 2 * n_frames bus values
+int mix_bus_admit(const mxb_exchange* ex, int n_frames, const char* who);
+// mix[t][c] = sum over w of partials[t][c][w] (W warps, n_frames frames) on `s`, summed over the ranks in rank order when
+// an exchange is attached; the same bits every run
+int mix_bus_reduce(mxb_exchange* ex, const double* partials, int W, int n_frames, double* mix, cudaStream_t s);
+// once `s` has been synchronised: MXB_ERR_STATE if a peer's part of a bus did not arrive within the exchange's time-out
+int mix_bus_status(mxb_exchange* ex, const char* who);
 
 }  // namespace mxb
-
-struct mxb_exchange {
-    mxb_ctx* ctx;
-    int rank, world, max_doubles;
-    size_t flags_bytes, slot_bytes;           // slot = world * max_doubles doubles, 128-byte multiple
-    unsigned char* local;                     // cudaMalloc'ed: flags + 2 slots
-    unsigned char* peers[mxb::kExchMaxWorld]; // cudaIpcOpenMemHandle'd (own entry = local)
-    bool connected;
-    unsigned long long seq;                   // calls so far
-    unsigned int* ticket;
-    unsigned int* status;                     // device word, see ExchDev::status
-    unsigned long long timeout_ns;            // default 5 s; MXB_EXCHANGE_TIMEOUT_MS overrides
-};
-
-namespace mxb {
-// fills the device descriptor for the next call and advances the sequence
-ExchDev exchange_next(mxb_exchange* ex);
-}

@@ -201,65 +201,6 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
     if (live) for (int i = 0; i < a.n_state; ++i) a.state[(size_t)i * V + (size_t)v] = st[i];
 }
 
-__global__ void patch_mix_reduce_kernel(const double* __restrict__ partials, double* __restrict__ mix, int W) {
-    // one CTA of 128 threads per (frame, channel) row: strided ascending sums, fixed tree -- the order never changes between runs
-    __shared__ double sm[4];
-    const double* p = partials + (size_t)blockIdx.x * (size_t)W;
-    double s = 0.0;
-    for (int w = threadIdx.x; w < W; w += blockDim.x) s += p[w];
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x == 0) mix[blockIdx.x] = (sm[0] + sm[1]) + (sm[2] + sm[3]);
-}
-
-// The same reduction with the cross-GPU exchange of the bus fused in (K6; protocol and buffers: exchange.cuh / exchange.cu, the bank's
-// twin of this kernel is mix_reduce_exchange_kernel in bank.cu): every CTA pushes its row sum into this rank's lane of EVERY rank's buffer
-// (posted NVLink stores), the last CTA to finish publishes one flag per peer, waits -- bounded -- for the peers' flags in its own buffer
-// and adds the world's buses in rank order: the same bits on every rank, every run.
-__global__ void patch_mix_reduce_exchange_kernel(const double* __restrict__ partials, double* __restrict__ mix, int rows, int W, const ExchDev x) {
-    __shared__ double sm[4];
-    __shared__ bool last;
-    const double* p = partials + (size_t)blockIdx.x * (size_t)W;
-    double s = 0.0;
-    for (int w = threadIdx.x; w < W; w += blockDim.x) s += p[w];
-#pragma unroll
-    for (int m = 16; m >= 1; m >>= 1) s += __shfl_xor_sync(0xffffffffu, s, m);
-    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
-    __syncthreads();
-    const double rowsum = (sm[0] + sm[1]) + (sm[2] + sm[3]);
-    if (threadIdx.x < x.world) x.dst_payload[threadIdx.x][blockIdx.x] = rowsum;      // thread r -> rank r's buffer
-    __threadfence_system();                           // this CTA's peer stores are ordered before its ticket
-    __syncthreads();
-    if (threadIdx.x == 0) last = atomicAdd(x.ticket, 1u) == gridDim.x - 1;
-    __syncthreads();
-    if (!last) return;
-    if (threadIdx.x < x.world) {
-        __threadfence_system();                       // cumulative: the other CTAs' stores were ordered before their tickets
-        asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(x.dst_flag[threadIdx.x]), "l"(x.seq1) : "memory");
-        const unsigned long long* flag = x.src_flags + (size_t)threadIdx.x * (kExchFlagBytes / sizeof(unsigned long long));
-        unsigned long long t0, t1, v;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-        unsigned spins = 0;
-        for (;;) {
-            asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(flag) : "memory");
-            if (v >= x.seq1) break;
-            if ((++spins & 1023u) == 0) {
-                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-                if (t1 - t0 > x.timeout_ns) { atomicOr(x.status, 1u << threadIdx.x); break; }      // a silent peer costs a time-out, not a hung box
-            }
-        }
-    }
-    if (threadIdx.x == 0) *x.ticket = 0;
-    __syncthreads();
-    for (int i = threadIdx.x; i < rows; i += blockDim.x) {
-        double t = 0.0;
-        for (int r = 0; r < x.world; ++r) t += __ldcg(x.src_payload + (size_t)r * (size_t)x.stride + i);
-        mix[i] = t;
-    }
-}
-
 int state_slots(const mxb_stage& g) { return patch_state_slots(g.op); }
 
 // MXB_PATCH_MODE=interpret | fused overrides the default (fused) for patches created afterwards: an A/B and debugging hook
@@ -501,9 +442,9 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
     MXB_REQUIRE(mem == MXB_MEM_HOST || mem == MXB_MEM_DEVICE, MXB_ERR_INVALID, "mxb_patch_process: mem %d", mem);
     MXB_REQUIRE(p->n_inputs == 0 || inputs, MXB_ERR_INVALID, "mxb_patch_process: the patch reads %d input streams, inputs is NULL", p->n_inputs);
     for (int i = 0; i < p->n_inputs; ++i) MXB_REQUIRE(inputs[i], MXB_ERR_INVALID, "mxb_patch_process: input stream %d is NULL", i);
-    if (mix && p->ex) {     // before any kernel runs: a refused call leaves every stage's state untouched
-        MXB_REQUIRE(p->ex->connected, MXB_ERR_STATE, "mxb_patch_process: the attached exchange is not connected to its peers");
-        MXB_REQUIRE(n_frames * 2 <= p->ex->max_doubles, MXB_ERR_INVALID, "mxb_patch_process: exchange holds %d values, the bus needs %d", p->ex->max_doubles, n_frames * 2);
+    if (mix) {     // before any kernel runs: a refused call leaves every stage's state untouched
+        const int rc = mix_bus_admit(p->ex, n_frames, "mxb_patch_process");
+        if (rc != MXB_OK) return rc;
     }
     if (n_frames == 0) return MXB_OK;
     DeviceGuard g(p->ctx->device);
@@ -517,33 +458,23 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
         a.in_kind[i] = (unsigned char)p->in_type[i];
         if (mem == MXB_MEM_HOST) {
             const size_t nb = patch_input_bytes(p->in_type[i], (size_t)n_frames, V);
-            if (nb > p->in_stage_len[i]) {
-                MXB_CUDA(cudaStreamSynchronize(s));
-                cudaFree(p->in_stage[i]); p->in_stage[i] = nullptr; p->in_stage_len[i] = 0;
-                cudaError_t e = cudaMalloc(&p->in_stage[i], nb);
-                if (e != cudaSuccess) { set_error("mxb_patch_process: staging cudaMalloc(%zu): %s", nb, cudaGetErrorString(e)); return MXB_ERR_ALLOC; }
-                p->in_stage_len[i] = nb;
-            }
+            const int rc = ensure(&p->in_stage[i], &p->in_stage_len[i], nb, s);
+            if (rc != MXB_OK) return rc;
             MXB_CUDA(cudaMemcpyAsync(p->in_stage[i], inputs[i], nb, cudaMemcpyHostToDevice, s));
             a.inputs[i] = p->in_stage[i];
         }
     }
     if (mem == MXB_MEM_HOST) {
         if (out) {
-            if (nb > p->out_stage_len) {
-                MXB_CUDA(cudaStreamSynchronize(s));
-                cudaFree(p->out_stage); p->out_stage = nullptr; p->out_stage_len = 0;
-                cudaError_t e = cudaMalloc((void**)&p->out_stage, nb);
-                if (e != cudaSuccess) { set_error("mxb_patch_process: staging cudaMalloc(%zu): %s", nb, cudaGetErrorString(e)); return MXB_ERR_ALLOC; }
-                p->out_stage_len = nb;
-            }
+            const int rc = ensure(&p->out_stage, &p->out_stage_len, (size_t)n_frames * V, s);
+            if (rc != MXB_OK) return rc;
             d_out = p->out_stage;
         }
         if (mix) d_mix = p->mix_dev;
     }
     const int grid = (int)((V + kPatchThreads - 1) / kPatchThreads);
     const int W = grid * (kPatchThreads / 32);
-    if (mix && !p->partials) { int rc = dev_alloc(&p->partials, (size_t)p->max_frames * 2 * (size_t)W, false); if (rc != MXB_OK) return rc; }
+    if (mix) { const int rc = ensure(&p->partials, &p->partials_len, (size_t)p->max_frames * 2 * (size_t)W, s); if (rc != MXB_OK) return rc; }
     a.V = p->V; a.n_frames = n_frames; a.n_stages = p->n_stages; a.n_params = p->n_params; a.n_state = p->n_state; a.W = W; a.taps = p->taps;
     a.sr = (double)(size_t)p->ctx->sample_rate;
     a.stages = p->d_stages; a.state_base = p->d_state_base; a.ring_of = p->d_ring_of; a.consts = p->d_consts;
@@ -564,27 +495,23 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
     }
     p->launches += 1;
     if (mix) {
-        if (p->ex) patch_mix_reduce_exchange_kernel<<<n_frames * 2, 128, 0, s>>>(p->partials, d_mix, n_frames * 2, W, exchange_next(p->ex));
-        else patch_mix_reduce_kernel<<<n_frames * 2, 128, 0, s>>>(p->partials, d_mix, W);
-        MXB_CUDA(cudaGetLastError());
+        const int rc = mix_bus_reduce(p->ex, p->partials, W, n_frames, d_mix, s);
+        if (rc != MXB_OK) return rc;
         p->launches += 1;
     }
     if (mem == MXB_MEM_HOST) {
         if (out) MXB_CUDA(cudaMemcpyAsync(out, d_out, nb, cudaMemcpyDeviceToHost, s));
         if (mix) MXB_CUDA(cudaMemcpyAsync(mix, d_mix, sizeof(double) * (size_t)n_frames * 2, cudaMemcpyDeviceToHost, s));
         MXB_CUDA(cudaStreamSynchronize(s));
-        if (mix && p->ex) {       // the call is synchronous in this mode: a timed-out exchange is an error of THIS call
-            unsigned int m = 0;
-            MXB_CUDA(cudaMemcpy(&m, p->ex->status, sizeof(m), cudaMemcpyDeviceToHost));
-            MXB_REQUIRE(m == 0, MXB_ERR_STATE, "mxb_patch_process: mix exchange timed out waiting for rank mask 0x%x (bus incomplete)", m);
-        }
+        if (mix) return mix_bus_status(p->ex, "mxb_patch_process");      // the call is synchronous in this mode: a timed-out exchange is an error of THIS call
     }
     return MXB_OK;
 }
 
 int32_t mxb_patch_set_exchange(mxb_patch* p, mxb_exchange* ex) {
     MXB_REQUIRE(p, MXB_ERR_INVALID, "mxb_patch_set_exchange: NULL patch");
-    if (ex) MXB_REQUIRE(ex->ctx->device == p->ctx->device, MXB_ERR_INVALID, "mxb_patch_set_exchange: exchange and patch live on different devices");
+    const int rc = mix_bus_attach(ex, p->ctx->device, "mxb_patch_set_exchange");
+    if (rc != MXB_OK) return rc;
     p->ex = ex;
     return MXB_OK;
 }

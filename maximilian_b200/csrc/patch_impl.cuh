@@ -270,10 +270,11 @@ struct mxb_patch {
     std::vector<double> consts;
     mxb_stage* d_stages; int* d_state_base; int* d_ring_of; double* d_consts;
     double* params; double* state; double* rings;
-    void* in_stage[mxb::kMaxInputs]; size_t in_stage_len[mxb::kMaxInputs];
+    unsigned char* in_stage[mxb::kMaxInputs]; size_t in_stage_len[mxb::kMaxInputs];      // staging for MXB_MEM_HOST input streams (bytes)
     int in_type[mxb::kMaxInputs];
     double* out_stage; size_t out_stage_len;
-    double* partials; double* mix_dev;
+    double* partials; size_t partials_len;
+    double* mix_dev;
     int eg_n, eg_loop, eg_retrigger; mxb::EgStage eg[mxb::kMaxEg];
     int64_t launches;
     int mode;              // MXB_PATCH_INTERPRET | MXB_PATCH_FUSED

@@ -366,6 +366,33 @@ def test_modulated_frequency_and_cutoff_with_envelope(port, filt):
         np.testing.assert_allclose(og, oo, rtol=1e-9, atol=1e-12)
 
 
+def test_host_staging_grows_with_the_block(port):
+    """Host-memory blocks of 16, 300, 40 and 512 frames through one bank (ADSR, lores, delay line) with every per-sample stream
+    (frequency, cutoff, trigger bytes, delay size), out and the bus: each staging buffer grows between blocks, and an fp32 block
+    followed by an fp64 block of the same length grows the output's by element size. Against the oracle at the bars of the
+    modulated tests (the swept cutoff is designed with libdevice: 1e-9); fp32 blocks are the oracle's output rounded to float32."""
+    from test_oracle_vs_reference import cutoff_sweeps, fm_frequencies
+    V, cap = 173, 128
+    p = W.voice_params(V, seed=71, delay_size=cap)
+    g = gpu_bank(V, osc="saw", filt="lores", env=True, delay=True, delay_capacity=cap, max_frames=512)
+    o = port.Bank(V, osc="saw", filt="lores", env=True, delay=True, delay_capacity=cap)
+    W.configure_bank(g, "lores", p, env=True, delay=True); W.configure_bank(o, "lores", p, env=True, delay=True)
+    blocks = [(16, np.float64), (300, np.float64), (40, np.float64), (512, np.float32), (512, np.float64)]
+    for blk, (B, dt) in enumerate(blocks):
+        f = fm_frequencies(V, B, blk); cu = cutoff_sweeps(V, B, blk); tv = trigger_bytes(V, B, blk, seed=11)
+        sz = np.floor(1 + (cap - 1) * np.random.default_rng(70 + blk).random((B, V)))
+        og, mg = g.process(B, freq_tv=f, cutoff_tv=cu, trig_tv=tv, delay_size_tv=sz, want_mix=True, out_dtype=dt)
+        oo, mo = o.process(B, freq_tv=f, cutoff_tv=cu, trig_tv=tv, delay_size_tv=sz, want_mix=True)
+        assert og.dtype == dt
+        # fp32: rounding to float32 (2^-24 relative) on top of the 1e-9 of the cutoff design
+        np.testing.assert_allclose(og, oo, rtol=1e-9 if dt == np.float64 else 2.0 ** -24 + 1e-9, atol=1e-12, err_msg=f"blk{blk} ({B} frames)")
+        np.testing.assert_allclose(mg, mo, rtol=1e-9, atol=1e-11, err_msg=f"blk{blk} ({B} frames)")
+        for s_ in ("delay_phase", "env_holdcount", "env_flags"):
+            assert np.array_equal(g.get(s_), o.get(s_)), (blk, s_)
+    for v in (0, 1, 31, 32, V // 2, V - 1):
+        np.testing.assert_allclose(g.ring(v, cap), o.ring(v, cap), rtol=1e-9, atol=1e-12, err_msg=f"ring of voice {v}")
+
+
 def test_play_block_is_the_interleaved_bus(port):
     """mxb_play_block = routing() of cpp/commandline/player.cpp:25-44: the interleaved RTAUDIO_FLOAT64 buffer of the next block."""
     V, B = 500, 256

@@ -181,6 +181,32 @@ def test_trigger_streams_as_bytes_and_as_packed_bits(mode, V):
 
 
 @pytest.mark.parametrize("mode", MODES)
+def test_host_staging_grows_with_the_block(port, mode):
+    """Host-memory blocks of 16, 300, 40 and 512 frames through one patch that reads a byte stream (trigger) and a double stream
+    (frequency) and writes out and the bus: the staging buffers of both inputs and of out grow between blocks. Bit-identical to
+    the oracle (saw, ADSR, * only), the bus within 1e-9."""
+    from maximilian_b200.patchdef import PatchDef, R
+    d = PatchDef()
+    d.stage("env_adsr", d.K(1.0), d.IN("trigger", "u8"), d.P("attack"), d.P("decay"), d.P("sustain"), d.P("release"), d.K(1.0), dst=R(0))
+    d.stage("osc", d.IN("freq"), kind="saw", dst=R(1))
+    d.stage("mul", R(1), R(0), dst=R(2))
+    d.stage("out", R(2)); d.stage("mix_stereo", R(2), d.P("pan"))
+    V = 333
+    prm = W.polysynth_params(V, seed=12); pat = W.note_pattern(V, seed=12)
+    g = capi.Patch(d, V, max_frames=512, mode=mode); o = port.Patch(d, V, kind="port")
+    for k in ("attack", "decay", "sustain", "release", "pan"):
+        g.set(k, prm[k]); o.set(k, prm[k])
+    rng = np.random.default_rng(12)
+    for blk, B in enumerate((16, 300, 40, 512)):
+        ins = {"trigger": W.note_triggers(pat, B, blk), "freq": rng.uniform(30.0, 3000.0, (B, V))}
+        og, mg = g.process(B, ins, want_mix=True); oo, mo = o.process(B, ins, want_mix=True)
+        _cmp(og, oo, True, f"blk{blk} ({B} frames)")
+        np.testing.assert_allclose(mg, mo, rtol=1e-9, atol=1e-10, err_msg=f"blk{blk} ({B} frames)")
+    for sl in range(SLOTS[2]):
+        _cmp(g.get_state(0, sl), o.get_state(0, sl), True, f"ADSR slot {sl}")
+
+
+@pytest.mark.parametrize("mode", MODES)
 @pytest.mark.parametrize("modulated", [False, True])
 def test_chorus_vs_oracle(port, mode, modulated):
     """maxiChorus as a stage (the noise it draws is an input stream): outputs 1e-9 (cos / sqrt of the per-sample or hoisted lores design
