@@ -281,7 +281,8 @@ enum {
     MXB_OP_ENV_ADSR,     /* maxiEnv::adsr(input, attack, decay, sustain, release, holdtime, trigger) src/maximilian.cpp:1362-1413:
                             src0 input, src1 trigger ((int)value == 1), src2..6 attack decay sustain release holdtime. state: amplitude, output, holdcount, flags */
     MXB_OP_ENV_AR,       /* maxiEnv::ar :1319-1358: src0 input, src1 trigger, src2 attack, src3 release, src4 holdtime */
-    MXB_OP_ENVGEN,       /* maxiEnvGen::play(trigger) src/maximilian.h:2276-2357, segments from mxb_patch_desc.eg_*: src0 trigger */
+    MXB_OP_ENVGEN,       /* maxiEnvGen::play(trigger) src/maximilian.h:2276-2357: src0 trigger. kind = index of the stage's envelope shape
+                            (mxb_patch_create2; mxb_patch_create: 0, the shape in mxb_patch_desc.eg_*) */
     MXB_OP_FILTER,       /* kind MXB_FILT_LORES | HIRES | LOPASS | HIPASS | BANDPASS: src0 input, src1 cutoff, src2 resonance */
     MXB_OP_SVF,          /* maxiSVF setCutoff + setResonance + play src/maximilian.h:1287-1334: src0 input, src1 cutoff, src2 resonance, src3..6 lp bp hp notch mix */
     MXB_OP_BIQUAD,       /* kind MXB_BQ_*: maxiBiquad::set + play src/maximilian.h:1360-1479: src0 input, src1 cutoff, src2 Q, src3 peakGain */
@@ -301,20 +302,29 @@ typedef struct { int32_t op, kind, dst, reserved; int32_t src[MXB_STAGE_SRCS]; }
 typedef struct {
     int32_t voices, n_stages, n_params, n_consts, n_inputs, max_frames;
     int32_t delay_taps;           /* ring slots per voice of every DELAY / FLANGER stage and of each of a CHORUS stage's two lines */
-    int32_t eg_stages, eg_loop, eg_retrigger;     /* maxiEnvGen::setup(levels, times, curves, looping, allowRetrigger): eg_stages + 1 levels */
+    int32_t eg_stages, eg_loop, eg_retrigger;     /* maxiEnvGen::setup(levels, times, curves, looping, allowRetrigger): eg_stages + 1 levels.
+                                                     The one shape of mxb_patch_create; empty (eg_stages 0) for mxb_patch_create2 */
     const mxb_stage* stages;
     const double* consts;
     const double *eg_levels, *eg_times /* ms or MXB_ENVGEN_HOLD */, *eg_curves;
     const int32_t* input_types;   /* n_inputs x MXB_IN_*, or NULL: every stream is doubles */
 } mxb_patch_desc;
 typedef struct mxb_patch mxb_patch;
+/* One maxiEnvGen shape: the arguments of maxiEnvGen::setup(levels, times, curves, looping, allowRetrigger), src/maximilian.h:2371-2402.
+ * stages + 1 levels, stages times (ms or MXB_ENVGEN_HOLD; at most one HOLD, as setup() requires) and stages curves. stages == 0 is a
+ * maxiEnvGen whose setup() was never called: it never triggers and plays 0. */
+typedef struct { int32_t stages, loop, retrigger; const double *levels, *times, *curves; } mxb_envgen_shape;
 /* The reference's lookup tables sineBuffer[514] and transition[1001] (src/maximilian.cpp:63, 67-200) are DATA of the
  * reference: an integration passes its own arrays (they have external linkage there). sine_before: the double that
  * maxiOsc::sinebuf4 reads at sineBuffer[-1] on the one sample per cycle where its phase has just wrapped into [-1, 0)
  * (an out-of-bounds read in the reference, src/maximilian.cpp:251); pass (&sineBuffer[0])[-1] for bit parity with a given
  * build, or sineBuffer[511] for the periodic extension the author intended. */
 int32_t mxb_ctx_set_tables(mxb_ctx* ctx, const double* sine514, const double* transition1001, double sine_before);
+/* mxb_patch_create: every MXB_OP_ENVGEN stage (kind 0) plays the one shape in desc->eg_*.
+ * mxb_patch_create2: one shape per maxiEnvGen object of the patch (an amp envelope and a filter envelope, ...): an ENVGEN stage plays
+ * shapes[kind], kind < n_shapes (0 .. 4). Stages may share a shape; each keeps its own state. desc->eg_stages must be 0. */
 int32_t mxb_patch_create(mxb_ctx* ctx, const mxb_patch_desc* desc, mxb_patch** patch);
+int32_t mxb_patch_create2(mxb_ctx* ctx, const mxb_patch_desc* desc, int32_t n_shapes, const mxb_envgen_shape* shapes, mxb_patch** patch);
 int32_t mxb_patch_destroy(mxb_patch* patch);
 int32_t mxb_patch_set_param(mxb_patch* patch, int32_t j, const double* values, int32_t mem);
 /* state slot `slot` of stage `stage` (the order given with the ops above; integral members arrive / return as doubles) */
@@ -330,7 +340,8 @@ int64_t mxb_patch_launch_count(const mxb_patch* patch);
  * the environment says MXB_PATCH_MODE=interpret. */
 int32_t mxb_patch_set_mode(mxb_patch* patch, int32_t mode);
 int32_t mxb_patch_get_mode(const mxb_patch* patch);
-/* The CUDA source the library generates for a descriptor (voices / max_frames are not looked at), NUL-terminated into buf[cap]
+/* The CUDA source the library generates for a descriptor (voices / max_frames / eg_* are not looked at: envelope shapes travel as kernel
+ * arguments, so one program serves every set of shapes; ENVGEN kinds 0 .. 3), NUL-terminated into buf[cap]
  * (may be NULL / 0); *needed = its size with the terminator. compile != 0 also runs it through NVRTC for sm_90a. Needs no device. */
 int32_t mxb_patch_codegen(const mxb_patch_desc* desc, char* buf, int64_t cap, int64_t* needed, int32_t compile);
 

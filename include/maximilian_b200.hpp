@@ -159,7 +159,7 @@ public:
         else if (!sameProgram()) throw maxiError(MXB_ERR_UNSUPPORTED, "maxiVoices: play() recorded a different patch than on the first block");
         if (bank_) runBank(nFrames, out, mix); else runPatch(nFrames, out, mix);
         prog_.clear(); consts_.clear(); nParams_ = 0; nInputs_ = 0; nextReg_ = 0; gate_ = maxiGate(); gateInput_ = -1; outSrc_ = MXB_NONE; lastSrc_ = MXB_NONE;
-        pendingPhase_.clear();
+        pendingPhase_.clear(); egObjs_.clear(); egShapes_.clear();
     }
 
     /* state read-back of a fused chain (checkpointing / tests): MXB_P_PHASE, MXB_S_* */
@@ -224,7 +224,20 @@ private:
     static bool blockConstant(int32_t s) { return s == MXB_NONE || (s >> 8) == 1 || (s >> 8) == 2; }   /* parameter or constant */
     bool sameProgram() const {
         return built_.size() == prog_.size() && std::memcmp(built_.data(), prog_.data(), sizeof(mxb_stage) * prog_.size()) == 0 &&
-               builtConsts_.size() == consts_.size() && std::memcmp(builtConsts_.data(), consts_.data(), sizeof(double) * consts_.size()) == 0;
+               builtConsts_.size() == consts_.size() && std::memcmp(builtConsts_.data(), consts_.data(), sizeof(double) * consts_.size()) == 0 &&
+               builtShapes_ == egShapes_;
+    }
+    /* the shape of one maxiEnvGen object (maxiEnvGen::setup, setLoop, setRetrigger) */
+    struct EgShape {
+        std::vector<double> levels, times, curves;
+        int loop = 0, retrigger = 0;
+        bool operator==(const EgShape& o) const { return levels == o.levels && times == o.times && curves == o.curves && loop == o.loop && retrigger == o.retrigger; }
+    };
+    /* the shape index of a maxiEnvGen object in this block: objects are numbered in the order they first play */
+    int32_t egShape(const void* obj, const EgShape& s) {
+        for (size_t i = 0; i < egObjs_.size(); ++i) if (egObjs_[i] == obj) return (int32_t)i;
+        egObjs_.push_back(obj); egShapes_.push_back(s);
+        return (int32_t)egObjs_.size() - 1;
     }
     std::vector<double> values(int32_t s) const {       /* a block-constant operand as a per-voice array */
         if ((s >> 8) == 1) return paramVals_[(size_t)(s & 0xff)];
@@ -291,11 +304,11 @@ private:
             d.voices = V_; d.n_stages = (int32_t)prog_.size(); d.n_params = nParams_; d.n_consts = (int32_t)consts_.size(); d.n_inputs = nInputs_;
             d.max_frames = maxFrames; d.delay_taps = delayCapacity_ > 0 ? delayCapacity_ : taps_;
             d.stages = prog_.data(); d.consts = consts_.data();
-            d.eg_stages = (int32_t)egTimes_.size(); d.eg_loop = egLoop_; d.eg_retrigger = egRetrigger_;
-            d.eg_levels = egLevels_.data(); d.eg_times = egTimes_.data(); d.eg_curves = egCurves_.data();
-            check(mxb_patch_create(ctx_, &d, &patch_), "mxb_patch_create");
+            std::vector<mxb_envgen_shape> shapes;
+            for (const EgShape& s : egShapes_) shapes.push_back({(int32_t)s.times.size(), s.loop, s.retrigger, s.levels.data(), s.times.data(), s.curves.data()});
+            check(mxb_patch_create2(ctx_, &d, (int32_t)shapes.size(), shapes.data(), &patch_), "mxb_patch_create2");
         }
-        built_ = prog_; builtConsts_ = consts_;
+        built_ = prog_; builtConsts_ = consts_; builtShapes_ = egShapes_;
         for (size_t j = 0; j < paramDirty_.size(); ++j) paramDirty_[j] = true;
     }
 
@@ -369,8 +382,8 @@ private:
     std::vector<const double*> inputPtr_;
     std::vector<double> gateStream_;
     std::vector<std::pair<int, std::vector<double>>> pendingPhase_;      /* maxiOsc::phaseReset: (stage, per-voice phase), applied before the block */
-    std::vector<double> egLevels_{0.0}, egTimes_, egCurves_;
-    int egLoop_ = 0, egRetrigger_ = 0;
+    std::vector<const void*> egObjs_;                                     /* the maxiEnvGen objects that played in this block, by shape index */
+    std::vector<EgShape> egShapes_, builtShapes_;
     std::vector<double> sine_, trans_; double sineBefore_ = 0.0; bool haveTables_ = false;
     int nParams_ = 0, nInputs_ = 0, nextReg_ = 0, gateInput_ = -1;
     int32_t outSrc_ = MXB_NONE, lastSrc_ = MXB_NONE;
@@ -527,25 +540,43 @@ private:
     std::vector<double> vec_[5];
 };
 
-/* maxiEnvGen, src/maximilian.h:2268-2547: one envelope shape for all voices, each with its own state */
+/* maxiEnvGen, src/maximilian.h:2268-2547: each object owns its envelope shape (levels, times, curves, loop, retrigger), played by all voices,
+ * each voice with its own state. An object whose setup() was never called plays 0, as in the reference. The shape is part of the patch: a
+ * shape changed after the first block is a different patch (maxiVoices::render throws). */
 class maxiEnvGen {
 public:
     static constexpr double HOLD = MXB_ENVGEN_HOLD;
     explicit maxiEnvGen(maxiVoices& v) : v_(&v) {}
     bool setup(const std::vector<double>& levels, const std::vector<double>& times, const std::vector<double>& curves, bool looping, bool allowRetrigger = false) {
         if (levels.size() != times.size() + 1 || levels.size() != curves.size() + 1) return false;
-        v_->egLevels_ = levels; v_->egTimes_ = times; v_->egCurves_ = curves; v_->egLoop_ = looping; v_->egRetrigger_ = allowRetrigger;
+        size_t n = times.size();
+        bool hold = false;
+        for (size_t i = 0; i < times.size() && n == times.size(); ++i) {
+            if (times[i] == HOLD && hold) n = i;
+            hold = hold || times[i] == HOLD;
+        }
+        /* the reference stops at a second HOLD segment (returns false), keeping the segments before it and the old loop / retrigger */
+        shape_.levels.assign(levels.begin(), levels.begin() + (long)n + 1);
+        shape_.times.assign(times.begin(), times.begin() + (long)n);
+        shape_.curves.assign(curves.begin(), curves.begin() + (long)n);
+        if (n < times.size()) return false;
+        shape_.loop = looping; shape_.retrigger = allowRetrigger;
         return true;
     }
+    void setLoop(const bool val) { shape_.loop = val; }
+    bool getLoop() { return shape_.loop != 0; }
+    void setRetrigger(const bool val) { shape_.retrigger = val; }
+    bool getRetrigger() { return shape_.retrigger != 0; }
     void setupAR(double attack, double release) { setup({0, 1, 0}, {attack, release}, {1, 1}, false, false); }
     void setupASR(double attack, double release) { setup({0, 1, 1, 0}, {attack, HOLD, release}, {1, 1, 1}, false, false); }
     void setupADSR(double attack, double decay, double sustain, double release) { setup({0, 1, sustain, sustain, 0}, {attack, decay, HOLD, release}, {1, 1, 1, 1}, false, false); }
-    template <class Trig> maxiSignal play(const Trig& trigger) { return v_->emit(MXB_OP_ENVGEN, 0, {trig(trigger)}); }
+    template <class Trig> maxiSignal play(const Trig& trigger) { const int32_t t = trig(trigger); return v_->emit(MXB_OP_ENVGEN, v_->egShape(this, shape_), {t}); }
 private:
     int32_t trig(const maxiSignal& s) { v_->check(s, "maxiEnvGen::play"); return s.src; }
     int32_t trig(const maxiStream& s) { return v_->operand(s); }
     int32_t trig(const maxiParam& p) { return v_->operand(p); }
     maxiVoices* v_;
+    maxiVoices::EgShape shape_;
 };
 
 /* maxiDelayline, src/maximilian.h:266-284 / src/maximilian.cpp:415-439 */

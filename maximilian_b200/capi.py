@@ -33,6 +33,7 @@ EXPORTS = [
     "mxb_octave_create", "mxb_octave_destroy", "mxb_octave_n_averages", "mxb_octave_config", "mxb_stft_process3",
     "mxb_ctx_set_tables", "mxb_patch_create", "mxb_patch_destroy", "mxb_patch_set_param", "mxb_patch_set_state", "mxb_patch_get_state",
     "mxb_patch_get_ring", "mxb_patch_process", "mxb_patch_launch_count", "mxb_patch_set_mode", "mxb_patch_get_mode", "mxb_patch_codegen",
+    "mxb_patch_create2",
 ]
 
 
@@ -133,6 +134,7 @@ def lib():
         "mxb_patch_set_mode": (i32, [vp, i32]),
         "mxb_patch_get_mode": (i32, [vp]),
         "mxb_patch_codegen": (i32, [vp, vp, i64, vp, i32]),
+        "mxb_patch_create2": (i32, [vp, vp, i32, vp, pp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = the library does not export a declared symbol
@@ -580,6 +582,26 @@ class PatchDesc(C.Structure):
                 ("input_types", C.POINTER(C.c_int32))]
 
 
+class EnvgenShape(C.Structure):
+    _fields_ = [("stages", C.c_int32), ("loop", C.c_int32), ("retrigger", C.c_int32),
+                ("levels", C.POINTER(C.c_double)), ("times", C.POINTER(C.c_double)), ("curves", C.POINTER(C.c_double))]
+
+
+def _doubles(x):
+    return (C.c_double * max(1, len(x)))(*x)
+
+
+def envgen_shapes(shapes):
+    """mxb_envgen_shape[] of (levels, times, curves, loop, retrigger) tuples; the second value keeps the arrays alive."""
+    arr = (EnvgenShape * max(1, len(shapes)))()
+    keep = [arr]
+    for i, (lv, tm, cv, loop, retrig) in enumerate(shapes):
+        a, b, c = _doubles(lv), _doubles(tm), _doubles(cv)
+        arr[i] = EnvgenShape(len(tm), int(loop), int(retrig), a, b, c)
+        keep += [a, b, c]
+    return arr, keep
+
+
 def set_tables(sine514, transition1001, sine_before, ctx=None, device=0, sample_rate=48000):
     """mxb_ctx_set_tables: the reference's sineBuffer / transition arrays (data of the reference, handed in by the caller)."""
     ctx = ctx or default_context(device, sample_rate)
@@ -609,7 +631,8 @@ def _patch_desc(defn, voices, max_frames, delay_taps):
         for k in range(8):
             st[i].src[k] = src[k]
     consts = (C.c_double * max(1, len(defn.consts)))(*defn.consts)
-    eg = defn.eg or ([0.0], [], [], False, False)
+    # one shape travels in the descriptor (mxb_patch_create); several go to mxb_patch_create2 (Patch) and the descriptor's eg_* stay empty
+    eg = defn.eg if defn.eg is not None and len(defn.shapes) == 1 else ([0.0], [], [], False, False)
     lv = (C.c_double * max(1, len(eg[0])))(*eg[0]); tm = (C.c_double * max(1, len(eg[1])))(*eg[1]); cv = (C.c_double * max(1, len(eg[2])))(*eg[2])
     ty = (C.c_int32 * max(1, len(defn.inputs)))(*[{"u8": 1, "bits": 2}.get(defn.input_types.get(n), 0) for n in defn.inputs])
     d = PatchDesc(int(voices), len(defn.stages), len(defn.params), len(defn.consts), len(defn.inputs), int(max_frames), int(delay_taps),
@@ -637,7 +660,11 @@ class Patch:
         self.defn, self.V, self.max_frames = defn, int(voices), int(max_frames)
         d, keep = _patch_desc(defn, self.V, self.max_frames, delay_taps)
         self.h = C.c_void_p()
-        check(lib().mxb_patch_create(self.ctx.h, C.byref(d), C.byref(self.h)), "mxb_patch_create")
+        if len(defn.shapes) <= 1:
+            check(lib().mxb_patch_create(self.ctx.h, C.byref(d), C.byref(self.h)), "mxb_patch_create")
+        else:
+            shapes, keep_shapes = envgen_shapes(defn.shapes)
+            check(lib().mxb_patch_create2(self.ctx.h, C.byref(d), len(defn.shapes), shapes, C.byref(self.h)), "mxb_patch_create2")
         if mode is not None:
             self.set_mode(mode)
 

@@ -31,6 +31,10 @@ struct Lane {
     __device__ __forceinline__ double& operator[](int slot) const { return base[slot * stride]; }
 };
 
+// MULTI_EG: the patch plays more than one maxiEnvGen shape. With one shape every ENVGEN stage plays shape 0, whose table and flags are then
+// read at fixed offsets of the argument block: a shape index read at run time makes ptxas spill in the stage loop, which cost the interpreter
+// about 2 % on the polysynth patch (H100 80GB HBM3, 700 W), a patch without any maxiEnvGen stage.
+template <bool MULTI_EG>
 __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a) {
     extern __shared__ double psm[];
     __shared__ mxb_stage s_stage[kMaxStages];
@@ -101,7 +105,8 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
                     q.envval = st[sb]; q.phase = (int)st[sb + 1]; q.state = (int)st[sb + 2]; q.nxc = st[sb + 3] != 0.0;
                     q.counter = (long long)st[sb + 4]; q.currentlevel = st[sb + 5];
                     q.tp = st[sb + 6]; q.tf = st[sb + 7]; q.hp = st[sb + 8]; q.hf = st[sb + 9]; q.rp = st[sb + 10]; q.rf = st[sb + 11];
-                    y = envgen_tick(q, fetch(g.src[0]), a.eg, a.eg_n, a.eg_loop, a.eg_retrigger);
+                    const int k = MULTI_EG ? g.kind : 0;
+                    y = envgen_tick(q, fetch(g.src[0]), a.eg[k], a.eg_n[k], a.eg_loop[k], a.eg_retrigger[k]);
                     st[sb] = q.envval; st[sb + 1] = (double)q.phase; st[sb + 2] = (double)q.state; st[sb + 3] = q.nxc ? 1.0 : 0.0;
                     st[sb + 4] = (double)q.counter; st[sb + 5] = q.currentlevel;
                     st[sb + 6] = q.tp; st[sb + 7] = q.tf; st[sb + 8] = q.hp; st[sb + 9] = q.hf; st[sb + 10] = q.rp; st[sb + 11] = q.rf;
@@ -223,58 +228,71 @@ bool src_ok(int s, const mxb_patch_desc* d) {
     }
 }
 
-}  // namespace
-
-extern "C" {
-
-int32_t mxb_ctx_set_tables(mxb_ctx* ctx, const double* sine514, const double* transition1001, double sine_before) {
-    MXB_REQUIRE(ctx && sine514 && transition1001, MXB_ERR_INVALID, "mxb_ctx_set_tables: NULL argument");
-    DeviceGuard g(ctx->device);
-    if (!ctx->d_sine) { int rc = dev_alloc(&ctx->d_sine, 514 + 1001); if (rc != MXB_OK) return rc; }
-    MXB_CUDA(cudaMemcpy(ctx->d_sine, sine514, sizeof(double) * 514, cudaMemcpyHostToDevice));
-    MXB_CUDA(cudaMemcpy(ctx->d_sine + 514, transition1001, sizeof(double) * 1001, cudaMemcpyHostToDevice));
-    ctx->sine_before = sine_before;
-    return MXB_OK;
+// maxiEnvGen::setup + setupSegmentTime, src/maximilian.h:2371-2402, 2524-2538: the segment table of one shape from levels / times / curves
+void eg_segments(const mxb_envgen_shape& s, const double srd, EgStage* eg) {
+    double accumulatedTime = 0;
+    for (int i = 0; i < s.stages; ++i) {
+        EgStage& e = eg[i];
+        e.startlevel = s.levels[i]; e.endlevel = s.levels[i + 1]; e.curve = s.curves[i]; e.pad = 0;
+        const double stageTime = s.times[i];
+        if (stageTime == MXB_ENVGEN_HOLD) { e.length = 0; e.hold = 1; e.gradient = 0; }
+        else {
+            const double len = ((stageTime / 1000.0) * srd) + accumulatedTime;
+            e.length = (long long)(size_t)floor(len);
+            accumulatedTime = len - e.length;
+            e.gradient = 1.0 / e.length;
+            e.hold = 0;
+        }
+    }
 }
 
-int32_t mxb_patch_create(mxb_ctx* ctx, const mxb_patch_desc* d, mxb_patch** out) {
-    MXB_REQUIRE(ctx && d && out && d->stages, MXB_ERR_INVALID, "mxb_patch_create: NULL argument");
+// mxb_patch_create and mxb_patch_create2: `who` names the entry point the caller used in the error messages
+int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shapes, const mxb_envgen_shape* shapes, mxb_patch** out, const char* who) {
+    MXB_REQUIRE(ctx && d && out && d->stages, MXB_ERR_INVALID, "%s: NULL argument", who);
     *out = nullptr;
-    MXB_REQUIRE(d->voices > 0 && d->max_frames > 0, MXB_ERR_INVALID, "mxb_patch_create: voices %d max_frames %d", d->voices, d->max_frames);
-    MXB_REQUIRE(d->n_stages > 0 && d->n_stages <= kMaxStages, MXB_ERR_INVALID, "mxb_patch_create: n_stages %d (1..%d)", d->n_stages, kMaxStages);
+    MXB_REQUIRE(d->voices > 0 && d->max_frames > 0, MXB_ERR_INVALID, "%s: voices %d max_frames %d", who, d->voices, d->max_frames);
+    MXB_REQUIRE(d->n_stages > 0 && d->n_stages <= kMaxStages, MXB_ERR_INVALID, "%s: n_stages %d (1..%d)", who, d->n_stages, kMaxStages);
     MXB_REQUIRE(d->n_params >= 0 && d->n_params <= kMaxParams && d->n_consts >= 0 && d->n_consts <= kMaxConsts && d->n_inputs >= 0 && d->n_inputs <= kMaxInputs,
-                MXB_ERR_INVALID, "mxb_patch_create: n_params %d n_consts %d n_inputs %d", d->n_params, d->n_consts, d->n_inputs);
-    MXB_REQUIRE(d->n_consts == 0 || d->consts, MXB_ERR_INVALID, "mxb_patch_create: consts is NULL");
-    MXB_REQUIRE(d->delay_taps >= 0, MXB_ERR_INVALID, "mxb_patch_create: delay_taps %d", d->delay_taps);
-    MXB_REQUIRE(d->eg_stages >= 0 && d->eg_stages <= kMaxEg, MXB_ERR_INVALID, "mxb_patch_create: eg_stages %d (0..%d)", d->eg_stages, kMaxEg);
+                MXB_ERR_INVALID, "%s: n_params %d n_consts %d n_inputs %d", who, d->n_params, d->n_consts, d->n_inputs);
+    MXB_REQUIRE(d->n_consts == 0 || d->consts, MXB_ERR_INVALID, "%s: consts is NULL", who);
+    MXB_REQUIRE(d->delay_taps >= 0, MXB_ERR_INVALID, "%s: delay_taps %d", who, d->delay_taps);
+    MXB_REQUIRE(n_shapes >= 0 && n_shapes <= kMaxEgShapes, MXB_ERR_INVALID, "%s: n_shapes %d (0..%d)", who, n_shapes, kMaxEgShapes);
+    MXB_REQUIRE(n_shapes == 0 || shapes, MXB_ERR_INVALID, "%s: shapes is NULL", who);
+    for (int k = 0; k < n_shapes; ++k) {
+        const mxb_envgen_shape& s = shapes[k];
+        MXB_REQUIRE(s.stages >= 0 && s.stages <= kMaxEg, MXB_ERR_INVALID, "%s: shape %d: stages %d (0..%d)", who, k, s.stages, kMaxEg);
+        MXB_REQUIRE(s.stages == 0 || (s.levels && s.times && s.curves), MXB_ERR_INVALID, "%s: shape %d needs levels / times / curves", who, k);
+        int holds = 0;
+        for (int i = 0; i < s.stages; ++i) holds += s.times[i] == MXB_ENVGEN_HOLD;
+        MXB_REQUIRE(holds <= 1, MXB_ERR_INVALID, "%s: shape %d has %d HOLD segments (maxiEnvGen::setup allows one)", who, k, holds);
+    }
     for (int i = 0; d->input_types && i < d->n_inputs; ++i)
-        MXB_REQUIRE(d->input_types[i] >= MXB_IN_F64 && d->input_types[i] <= MXB_IN_BITS, MXB_ERR_INVALID, "mxb_patch_create: input_types[%d] = %d", i, d->input_types[i]);
+        MXB_REQUIRE(d->input_types[i] >= MXB_IN_F64 && d->input_types[i] <= MXB_IN_BITS, MXB_ERR_INVALID, "%s: input_types[%d] = %d", who, i, d->input_types[i]);
     int n_state = 0, n_rings = 0;
-    bool tables = false, eg = false;
+    bool tables = false;
     for (int i = 0; i < d->n_stages; ++i) {
         const mxb_stage& g = d->stages[i];
-        MXB_REQUIRE(g.op >= MXB_OP_OSC && g.op <= MXB_OP_CHORUS, MXB_ERR_INVALID, "mxb_patch_create: stage %d: unknown op %d", i, g.op);
-        MXB_REQUIRE(g.dst == MXB_NONE || (g.dst >= 0 && g.dst < kMaxRegs), MXB_ERR_INVALID, "mxb_patch_create: stage %d: dst %d", i, g.dst);
-        for (int k = 0; k < MXB_STAGE_SRCS; ++k) MXB_REQUIRE(src_ok(g.src[k], d), MXB_ERR_INVALID, "mxb_patch_create: stage %d: operand %d = 0x%x", i, k, g.src[k]);
+        MXB_REQUIRE(g.op >= MXB_OP_OSC && g.op <= MXB_OP_CHORUS, MXB_ERR_INVALID, "%s: stage %d: unknown op %d", who, i, g.op);
+        MXB_REQUIRE(g.dst == MXB_NONE || (g.dst >= 0 && g.dst < kMaxRegs), MXB_ERR_INVALID, "%s: stage %d: dst %d", who, i, g.dst);
+        for (int k = 0; k < MXB_STAGE_SRCS; ++k) MXB_REQUIRE(src_ok(g.src[k], d), MXB_ERR_INVALID, "%s: stage %d: operand %d = 0x%x", who, i, k, g.src[k]);
         if (g.op == MXB_OP_OSC) {
-            MXB_REQUIRE(g.kind >= MXB_OSC_SINEWAVE && g.kind <= MXB_OSC_SAWN, MXB_ERR_INVALID, "mxb_patch_create: stage %d: osc kind %d", i, g.kind);
+            MXB_REQUIRE(g.kind >= MXB_OSC_SINEWAVE && g.kind <= MXB_OSC_SAWN, MXB_ERR_INVALID, "%s: stage %d: osc kind %d", who, i, g.kind);
             tables = tables || g.kind >= MXB_OSC_SINEBUF;
         }
         if (g.op == MXB_OP_FILTER) MXB_REQUIRE(g.kind == MXB_FILT_LORES || g.kind == MXB_FILT_HIRES || g.kind == MXB_FILT_LOPASS || g.kind == MXB_FILT_HIPASS || g.kind == MXB_FILT_BANDPASS,
-                                               MXB_ERR_INVALID, "mxb_patch_create: stage %d: filter kind %d", i, g.kind);
-        if (g.op == MXB_OP_BIQUAD) MXB_REQUIRE(g.kind >= MXB_BQ_LOWPASS && g.kind <= MXB_BQ_HIGHSHELF, MXB_ERR_INVALID, "mxb_patch_create: stage %d: biquad type %d", i, g.kind);
-        if (g.op == MXB_OP_NONLIN) MXB_REQUIRE(g.kind >= MXB_NL_ATANDIST && g.kind <= MXB_NL_FASTATAN, MXB_ERR_INVALID, "mxb_patch_create: stage %d: nonlinearity %d", i, g.kind);
-        if (patch_stage_rings(g.op)) { MXB_REQUIRE(d->delay_taps > 0, MXB_ERR_INVALID, "mxb_patch_create: stage %d needs delay_taps > 0", i); n_rings += patch_stage_rings(g.op); }
-        if (g.op == MXB_OP_ENVGEN) eg = true;
+                                               MXB_ERR_INVALID, "%s: stage %d: filter kind %d", who, i, g.kind);
+        if (g.op == MXB_OP_BIQUAD) MXB_REQUIRE(g.kind >= MXB_BQ_LOWPASS && g.kind <= MXB_BQ_HIGHSHELF, MXB_ERR_INVALID, "%s: stage %d: biquad type %d", who, i, g.kind);
+        if (g.op == MXB_OP_NONLIN) MXB_REQUIRE(g.kind >= MXB_NL_ATANDIST && g.kind <= MXB_NL_FASTATAN, MXB_ERR_INVALID, "%s: stage %d: nonlinearity %d", who, i, g.kind);
+        if (g.op == MXB_OP_ENVGEN) MXB_REQUIRE(g.kind >= 0 && g.kind < n_shapes, MXB_ERR_INVALID, "%s: stage %d: envelope shape %d of %d", who, i, g.kind, n_shapes);
+        if (patch_stage_rings(g.op)) { MXB_REQUIRE(d->delay_taps > 0, MXB_ERR_INVALID, "%s: stage %d needs delay_taps > 0", who, i); n_rings += patch_stage_rings(g.op); }
         n_state += state_slots(g);
     }
-    if (tables) MXB_REQUIRE(ctx->d_sine, MXB_ERR_STATE, "mxb_patch_create: sinebuf / sinebuf4 / sawn need the reference's tables: call mxb_ctx_set_tables first");
-    if (eg) MXB_REQUIRE(d->eg_stages > 0 && d->eg_levels && d->eg_times && d->eg_curves, MXB_ERR_INVALID, "mxb_patch_create: an ENVGEN stage needs eg_levels / eg_times / eg_curves");
+    if (tables) MXB_REQUIRE(ctx->d_sine, MXB_ERR_STATE, "%s: sinebuf / sinebuf4 / sawn need the reference's tables: call mxb_ctx_set_tables first", who);
     const size_t per_thread = (size_t)(kMaxRegs + d->n_params + n_state);
-    MXB_REQUIRE(per_thread * 8 * kPatchThreads <= 200 * 1024, MXB_ERR_UNSUPPORTED, "mxb_patch_create: %zu doubles of registers, parameters and state per voice do not fit shared memory", per_thread);
+    MXB_REQUIRE(per_thread * 8 * kPatchThreads <= 200 * 1024, MXB_ERR_UNSUPPORTED, "%s: %zu doubles of registers, parameters and state per voice do not fit shared memory", who, per_thread);
     DeviceGuard g(ctx->device);
     mxb_patch* p = new (std::nothrow) mxb_patch();
-    MXB_REQUIRE(p, MXB_ERR_ALLOC, "mxb_patch_create: out of host memory");
+    MXB_REQUIRE(p, MXB_ERR_ALLOC, "%s: out of host memory", who);
     p->ctx = ctx; p->V = d->voices; p->n_stages = d->n_stages; p->n_params = d->n_params; p->n_consts = d->n_consts; p->n_inputs = d->n_inputs;
     p->max_frames = d->max_frames; p->taps = d->delay_taps; p->n_state = n_state; p->n_rings = n_rings;
     p->stages.assign(d->stages, d->stages + d->n_stages);
@@ -288,24 +306,10 @@ int32_t mxb_patch_create(mxb_ctx* ctx, const mxb_patch_desc* d, mxb_patch** out)
         p->ring_of.push_back(nr ? ri : -1);
         ri += nr;
     }
-    // maxiEnvGen::setup + setupSegmentTime, src/maximilian.h:2371-2402, 2524-2538: segment table from levels / times / curves
-    p->eg_n = d->eg_stages; p->eg_loop = d->eg_loop; p->eg_retrigger = d->eg_retrigger;
-    {
-        double accumulatedTime = 0;
-        const double srd = (double)(size_t)ctx->sample_rate;
-        for (int i = 0; i < d->eg_stages; ++i) {
-            EgStage& s = p->eg[i];
-            s.startlevel = d->eg_levels[i]; s.endlevel = d->eg_levels[i + 1]; s.curve = d->eg_curves[i]; s.pad = 0;
-            const double stageTime = d->eg_times[i];
-            if (stageTime == MXB_ENVGEN_HOLD) { s.length = 0; s.hold = 1; s.gradient = 0; }
-            else {
-                const double len = ((stageTime / 1000.0) * srd) + accumulatedTime;
-                s.length = (long long)(size_t)floor(len);
-                accumulatedTime = len - s.length;
-                s.gradient = 1.0 / s.length;
-                s.hold = 0;
-            }
-        }
+    p->n_shapes = n_shapes;
+    for (int k = 0; k < n_shapes; ++k) {
+        p->eg_n[k] = shapes[k].stages; p->eg_loop[k] = shapes[k].loop; p->eg_retrigger[k] = shapes[k].retrigger;
+        eg_segments(shapes[k], (double)(size_t)ctx->sample_rate, p->eg[k]);
     }
     const size_t V = (size_t)p->V;
     int rc = MXB_OK;
@@ -327,10 +331,43 @@ int32_t mxb_patch_create(mxb_ctx* ctx, const mxb_patch_desc* d, mxb_patch** out)
         for (int k = 6; k < 12 && e == cudaSuccess; ++k)
             e = cudaMemcpy(p->state + (size_t)(p->state_base[i] + k) * V, ones.data(), sizeof(double) * V, cudaMemcpyHostToDevice);
     }
-    if (e != cudaSuccess) { set_error("mxb_patch_create: %s", cudaGetErrorString(e)); mxb_patch_destroy(p); return MXB_ERR_CUDA; }
+    if (e != cudaSuccess) { set_error("%s: %s", who, cudaGetErrorString(e)); mxb_patch_destroy(p); return MXB_ERR_CUDA; }
 #undef TRY
     *out = p;
     return MXB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t mxb_ctx_set_tables(mxb_ctx* ctx, const double* sine514, const double* transition1001, double sine_before) {
+    MXB_REQUIRE(ctx && sine514 && transition1001, MXB_ERR_INVALID, "mxb_ctx_set_tables: NULL argument");
+    DeviceGuard g(ctx->device);
+    if (!ctx->d_sine) { int rc = dev_alloc(&ctx->d_sine, 514 + 1001); if (rc != MXB_OK) return rc; }
+    MXB_CUDA(cudaMemcpy(ctx->d_sine, sine514, sizeof(double) * 514, cudaMemcpyHostToDevice));
+    MXB_CUDA(cudaMemcpy(ctx->d_sine + 514, transition1001, sizeof(double) * 1001, cudaMemcpyHostToDevice));
+    ctx->sine_before = sine_before;
+    return MXB_OK;
+}
+
+int32_t mxb_patch_create(mxb_ctx* ctx, const mxb_patch_desc* d, mxb_patch** out) {
+    MXB_REQUIRE(d, MXB_ERR_INVALID, "mxb_patch_create: NULL argument");
+    MXB_REQUIRE(d->eg_stages >= 0 && d->eg_stages <= kMaxEg, MXB_ERR_INVALID, "mxb_patch_create: eg_stages %d (0..%d)", d->eg_stages, kMaxEg);
+    bool eg = false;
+    for (int i = 0; d->stages && i < d->n_stages && i < kMaxStages; ++i) eg = eg || d->stages[i].op == MXB_OP_ENVGEN;
+    if (eg) MXB_REQUIRE(d->eg_stages > 0 && d->eg_levels && d->eg_times && d->eg_curves, MXB_ERR_INVALID, "mxb_patch_create: an ENVGEN stage needs eg_levels / eg_times / eg_curves");
+    // the descriptor's shape is shape 0 of mxb_patch_create2
+    const mxb_envgen_shape shape = {d->eg_stages, d->eg_loop, d->eg_retrigger, d->eg_levels, d->eg_times, d->eg_curves};
+    mxb_patch_desc d2 = *d;
+    d2.eg_stages = 0; d2.eg_levels = d2.eg_times = d2.eg_curves = nullptr;
+    return create_patch(ctx, &d2, d->eg_stages > 0 ? 1 : 0, &shape, out, "mxb_patch_create");
+}
+
+int32_t mxb_patch_create2(mxb_ctx* ctx, const mxb_patch_desc* d, int32_t n_shapes, const mxb_envgen_shape* shapes, mxb_patch** out) {
+    MXB_REQUIRE(d, MXB_ERR_INVALID, "mxb_patch_create2: NULL argument");
+    MXB_REQUIRE(d->eg_stages == 0, MXB_ERR_INVALID, "mxb_patch_create2: the descriptor's eg_* must be empty (eg_stages %d): the shapes come in `shapes`", d->eg_stages);
+    return create_patch(ctx, d, n_shapes, shapes, out, "mxb_patch_create2");
 }
 
 int32_t mxb_patch_destroy(mxb_patch* p) {
@@ -417,6 +454,7 @@ int32_t mxb_patch_codegen(const mxb_patch_desc* d, char* buf, int64_t cap, int64
         const mxb_stage& g = d->stages[i];
         MXB_REQUIRE(g.op >= MXB_OP_OSC && g.op <= MXB_OP_CHORUS && (g.dst == MXB_NONE || (g.dst >= 0 && g.dst < kMaxRegs)), MXB_ERR_INVALID, "mxb_patch_codegen: stage %d", i);
         for (int k = 0; k < MXB_STAGE_SRCS; ++k) MXB_REQUIRE(src_ok(g.src[k], d), MXB_ERR_INVALID, "mxb_patch_codegen: stage %d: operand %d = 0x%x", i, k, g.src[k]);
+        if (g.op == MXB_OP_ENVGEN) MXB_REQUIRE(g.kind >= 0 && g.kind < kMaxEgShapes, MXB_ERR_INVALID, "mxb_patch_codegen: stage %d: envelope shape %d (0..%d)", i, g.kind, kMaxEgShapes - 1);
     }
     int types[kMaxInputs] = {};
     for (int i = 0; d->input_types && i < d->n_inputs; ++i) {
@@ -480,8 +518,8 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
     a.stages = p->d_stages; a.state_base = p->d_state_base; a.ring_of = p->d_ring_of; a.consts = p->d_consts;
     a.params = p->params; a.state = p->state; a.out = d_out; a.partials = mix ? p->partials : nullptr; a.rings = p->rings;
     a.sine = p->ctx->d_sine; a.transition = p->ctx->d_sine ? p->ctx->d_sine + 514 : nullptr; a.sine_before = p->ctx->sine_before;
-    a.eg_n = p->eg_n; a.eg_loop = p->eg_loop; a.eg_retrigger = p->eg_retrigger;
-    for (int i = 0; i < p->eg_n; ++i) a.eg[i] = p->eg[i];
+    memcpy(a.eg_n, p->eg_n, sizeof(a.eg_n)); memcpy(a.eg_loop, p->eg_loop, sizeof(a.eg_loop)); memcpy(a.eg_retrigger, p->eg_retrigger, sizeof(a.eg_retrigger));
+    memcpy(a.eg, p->eg, sizeof(a.eg));
     if (p->mode == MXB_PATCH_FUSED) {
         // the kernel generated for this stage list (patch_fuse.cu): compiled on first use, then launched like any other
         int rc = patch_fused_load(p);
@@ -489,8 +527,9 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
         if (rc != MXB_OK) return rc;
     } else {
         const size_t smem = sizeof(double) * (size_t)(kMaxRegs + p->n_params + p->n_state) * kPatchThreads;
-        MXB_CUDA(cudaFuncSetAttribute(patch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        patch_kernel<<<grid, kPatchThreads, smem, s>>>(a);
+        void (*kernel)(const PatchArgs) = p->n_shapes > 1 ? patch_kernel<true> : patch_kernel<false>;
+        MXB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kernel<<<grid, kPatchThreads, smem, s>>>(a);
         MXB_CUDA(cudaGetLastError());
     }
     p->launches += 1;

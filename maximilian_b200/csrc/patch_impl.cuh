@@ -13,6 +13,7 @@ namespace mxb {
 
 constexpr int kPatchThreads = 128;
 constexpr int kMaxStages = 64, kMaxParams = 32, kMaxConsts = 64, kMaxInputs = 8, kMaxRegs = 16, kMaxEg = 16;
+constexpr int kMaxEgShapes = 4;          // maxiEnvGen shapes of one patch (9.Envelopes2 plays three); their segment tables are kernel arguments
 
 struct EgStage { double startlevel, endlevel, gradient, curve; long long length; int hold; int pad; };
 
@@ -33,9 +34,10 @@ struct PatchArgs {
     const double* sine;              // sineBuffer[514], src/maximilian.cpp:63
     const double* transition;        // transition[1001], src/maximilian.cpp:67-200
     double sine_before;              // what sinebuf4 reads at sineBuffer[-1] on its wrap sample (out of bounds in the reference)
-    int eg_n, eg_loop, eg_retrigger;
-    EgStage eg[kMaxEg];
+    int eg_n[kMaxEgShapes], eg_loop[kMaxEgShapes], eg_retrigger[kMaxEgShapes];      // shape k: an ENVGEN stage of kind k plays it
+    EgStage eg[kMaxEgShapes][kMaxEg];
 };
+static_assert(sizeof(PatchArgs) <= 4096, "PatchArgs must fit the 4 KB kernel parameter block");
 
 // table oscillators, src/maximilian.cpp:237-274, 342-359
 __device__ __forceinline__ double osc_table_tick(const int kind, double& phase, double& output, const double frequency, const double sr,
@@ -275,7 +277,9 @@ struct mxb_patch {
     double* out_stage; size_t out_stage_len;
     double* partials; size_t partials_len;
     double* mix_dev;
-    int eg_n, eg_loop, eg_retrigger; mxb::EgStage eg[mxb::kMaxEg];
+    int n_shapes;          // maxiEnvGen shapes; ENVGEN stage kinds index them
+    int eg_n[mxb::kMaxEgShapes], eg_loop[mxb::kMaxEgShapes], eg_retrigger[mxb::kMaxEgShapes];
+    mxb::EgStage eg[mxb::kMaxEgShapes][mxb::kMaxEg];
     int64_t launches;
     int mode;              // MXB_PATCH_INTERPRET | MXB_PATCH_FUSED
     mxb_fused* fused;      // compiled on the first fused launch

@@ -29,7 +29,7 @@ class PatchDef:
         self.params = []          # names, index = parameter slot
         self.inputs = []          # names, index = input stream
         self.input_types = {}     # name -> "u8" | "bits" for byte / packed-bit streams (triggers, gates); doubles otherwise
-        self.eg = None            # (levels, times, curves, loop, retrigger)
+        self.eg = None            # maxiEnvGen shape 0: (levels, times, curves, loop, retrigger)
 
     def K(self, value):
         """scalar constant operand (deduplicated by bit pattern)"""
@@ -66,6 +66,24 @@ class PatchDef:
         self.stages.append((OP[op], k, dst, s))
         return len(self.stages) - 1
 
+    # shapes 1, 2, ... of a patch with several maxiEnvGen shapes; an instance attribute from the second shape on, so that a PatchDef
+    # with one shape has exactly the attributes it always had (the oracle's recorded reference calls digest a PatchDef by them)
+    eg_more = ()
+
     def envgen(self, levels, times, curves, loop=False, retrigger=False):
+        """A maxiEnvGen shape: the arguments of maxiEnvGen::setup(levels, times, curves, looping, allowRetrigger). Returns its index, the
+        `kind` of the envgen stages that play it (stage("envgen", trigger, kind=i)). One level and no times / curves: a maxiEnvGen whose
+        setup() was never called (it plays 0)."""
         assert len(levels) == len(times) + 1 == len(curves) + 1
-        self.eg = (list(map(float, levels)), list(map(float, times)), list(map(float, curves)), bool(loop), bool(retrigger))
+        shape = (list(map(float, levels)), list(map(float, times)), list(map(float, curves)), bool(loop), bool(retrigger))
+        if self.eg is None:
+            self.eg = shape
+            return 0
+        self.eg_more = list(self.eg_more) + [shape]
+        assert len(self.shapes) <= 4
+        return len(self.eg_more)
+
+    @property
+    def shapes(self):
+        """every maxiEnvGen shape, in index order"""
+        return ([self.eg] if self.eg is not None else []) + list(self.eg_more)
