@@ -384,7 +384,13 @@ int32_t mxb_env_coeffs(int32_t kind, const double* ms, int64_t n, int32_t sample
  * time-major like a bank's out: stride_c = 1, stride_t = channels).
  * Frame f of channel c is written at ((c*max_frames) + f)*bins of mags/phases/re/im (each optional)
  * and at ((c*max_frames) + f)*num_coeffs of coeffs when an mfcc handle is given (fused: the spectrum
- * never leaves the chip unless asked for). *n_frames receives the frames fired per channel. */
+ * never leaves the chip unless asked for). *n_frames receives the frames fired per channel.
+ * Input contract: samples are finite with |x| < 2^48. Then |X_k| <= fft_size * max|x| (1024 * max|x| < 2^58
+ * for the 1024-point kernel, < 2^59 at 2048), the power |X_k|^2 < 2^118 stays below FLT_MAX (~2^128) and no
+ * magnitude overflows. The fused 1024-point MFCC
+ * (K4s) relies on it: it does not look for non-finite magnitudes. The other sizes, and mxb_mfcc_process on
+ * caller-supplied magnitudes, follow the reference there too: a NaN anywhere in a frame, or an inf at a bin
+ * where a band has zero weight, makes that band 0 (the reference's band is NaN, and its > 1e-6 gate fails). */
 int32_t mxb_stft_create(mxb_ctx* ctx, int32_t channels, int32_t fft_size, int32_t hop_size, mxb_stft** st);
 int32_t mxb_stft_destroy(mxb_stft* st);
 int32_t mxb_stft_process(mxb_stft* st, const float* in, int64_t stride_c, int64_t stride_t, int32_t n_samples,

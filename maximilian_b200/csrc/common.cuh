@@ -87,6 +87,7 @@ struct mxb_ctx {
     int sample_rate;
     int sm_count;
     int cc_major, cc_minor;
+    int smem_optin;          // cudaDevAttrMaxSharedMemoryPerBlockOptin: the most shared memory one CTA may opt in to
     double* d_sine;          // sineBuffer[514] ++ transition[1001] of the reference (mxb_ctx_set_tables), or NULL
     double sine_before;
 };

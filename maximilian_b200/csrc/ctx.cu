@@ -38,12 +38,15 @@ int32_t mxb_ctx_create(int32_t device, int32_t sample_rate, mxb_ctx** out) {
     mxb::DeviceGuard g(device);
     MXB_REQUIRE(g.ok, MXB_ERR_CUDA, "mxb_ctx_create: cudaSetDevice(%d) failed", device);
     MXB_CUDA(cudaFree(0));
+    int smem_optin = 0;
+    MXB_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
     mxb_ctx* c = new mxb_ctx();
     c->device = device;
     c->sample_rate = sample_rate;
     c->sm_count = prop.multiProcessorCount;
     c->cc_major = prop.major;
     c->cc_minor = prop.minor;
+    c->smem_optin = smem_optin;
     c->d_sine = nullptr; c->sine_before = 0.0;
     *out = c;
     return MXB_OK;

@@ -79,8 +79,10 @@ __device__ __forceinline__ void dmma_tile(const double* __restrict__ ap, const d
 // arguments between e^-40 and e^41 and around 1). The argument reduction and the degree-14 polynomial in s = f / (2 + f) are the
 // classic ones (x = 2^k (1 + f), sqrt(2)/2 < 1 + f < sqrt(2); log(1 + f) = f - f^2/2 + s (f^2/2 + R(s^2))); the quotient comes from a
 // single-precision reciprocal refined twice. About 40 straight-line instructions against libdevice's ~90 with branches: two calls next
-// to each other interleave. Only the mel stage uses it: its arguments are squares > 1e-12.
+// to each other interleave. Only the mel stage uses it: its arguments are squares > 1e-12, or +inf (log(+inf) = +inf, like libm; the
+// reduction below would read the exponent field of +inf as 2^1024 and return 1024 ln 2).
 __device__ __forceinline__ double log_pos(double x) {
+    const double x0 = x;
     int hx = __double2hiint(x);
     const int lx = __double2loint(x);
     int kexp = (hx >> 20) - 1023;
@@ -101,7 +103,8 @@ __device__ __forceinline__ double log_pos(double x) {
                                             6.666666666666735130e-01));
     const double R = __dadd_rn(t2, t1), hfsq = __dmul_rn(__dmul_rn(0.5, f), f);
     const double lo = __fma_rn(s, __dadd_rn(hfsq, R), __dmul_rn(dk, 1.90821492927058770002e-10));
-    return __dsub_rn(__dmul_rn(dk, 6.93147180369123816490e-01), __dsub_rn(__dsub_rn(hfsq, lo), f));
+    const double y = __dsub_rn(__dmul_rn(dk, 6.93147180369123816490e-01), __dsub_rn(__dsub_rn(hfsq, lo), f));
+    return x0 == (double)INFINITY ? x0 : y;
 }
 
 __device__ __forceinline__ u64 pk2(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }

@@ -312,13 +312,34 @@ def test_stft_frame_schedule(port):
     assert s.process(np.zeros((1, 1), dtype=np.float32))["mags"].shape[1] == 1
 
 
-@pytest.mark.parametrize("cfg", [(512, 42, 40, 20.0, 20000.0, 48000), (512, 42, 13, 20.0, 20000.0, 44100),
-                                 (512, 256, 13, 20.0, 20000.0, 48000), (256, 20, 12, 100.0, 8000.0, 48000)])
+# the shapes the GPU's fused paths are checked at (tests/test_gpu_spectral_epilogues.py): filter / coefficient counts that change the
+# tensor-core tiling, band limits that move the bank's last bin, the 64 / 128 / 1024-bin banks of 128 / 256 / 2048-point transforms
+MFCC_SHAPES = [(512, 42, 40, 20.0, 20000.0, 48000), (512, 42, 13, 20.0, 20000.0, 44100),
+               (512, 256, 13, 20.0, 20000.0, 48000), (256, 20, 12, 100.0, 8000.0, 48000),
+               (512, 40, 13, 20.0, 20000.0, 48000), (512, 32, 32, 20.0, 20000.0, 48000), (512, 24, 30, 300.0, 24000.0, 48000),
+               (512, 3, 5, 20.0, 20000.0, 48000), (512, 1, 1, 20.0, 20000.0, 48000), (512, 26, 13, 2000.0, 8000.0, 16000),
+               (512, 64, 20, 0.0, 24000.0, 48000), (512, 520, 13, 20.0, 20000.0, 48000),
+               (64, 16, 13, 20.0, 20000.0, 48000), (128, 26, 13, 20.0, 20000.0, 44100), (1024, 42, 40, 20.0, 20000.0, 48000)]
+
+
+def mfcc_bad_bins(cfg):
+    """Bins for the non-finite rows of an MFCC test: one inside the bank's bands (the middle of its frequency range; the reference's
+    bin spacing is sr / numBins) and the top bin, where no band has weight."""
+    bins, _, _, fmin, fmax, sr = cfg
+    return int((fmin + min(fmax, sr / 2)) / 2 / (sr / bins)), bins - 1
+
+
+@pytest.mark.parametrize("cfg", MFCC_SHAPES)
 def test_mfcc_bit_exact(port, reference, cfg):
     bins = cfg[0]
     st = port.Stft(3, 2 * bins, bins)
     mags = st.process(W.channel_streams(3, 2 * bins * 8, seed=bins))["mags"]
     mags[0, 0] = 0.0                                   # silent frame: log gate (> 1e-6) takes the 0 branch
+    # non-finite magnitudes: the reference sums weight * magnitude over every bin, so 0 * NaN and 0 * inf make a band NaN (-> 0)
+    inside, above = mfcc_bad_bins(cfg)
+    mags[2, 0, 5] = np.nan
+    mags[2, 1, inside] = np.inf
+    mags[2, 2, above] = np.inf
     a = port.Mfcc(*cfg, kind="port"); b = reference.Mfcc(*cfg, kind="reference")
     ca, ma = a.process(mags); cb, mb = b.process(mags)
     assert _same(ma, mb)
@@ -327,15 +348,16 @@ def test_mfcc_bit_exact(port, reference, cfg):
 
 
 def test_spectral_features_bit_exact(port, reference):
-    # maxiFFT::magsToDB / spectralFlatness / spectralCentroid, src/libs/maxiFFT.cpp:101-132
-    mags = port.Stft(3, 1024, 512).process(W.channel_streams(3, 8192, seed=8))["mags"]
-    mags[0, 0] = 0.0                                  # all-zero frame: both features return 0
-    mags[1, 1, :7] = 0.0                              # zeros are skipped by the geometric mean
-    for sr in (44100, 48000):
-        a = port.spectral_features(mags, 1024, sr, kind="port")
-        b = reference.spectral_features(mags, 1024, sr, kind="reference")
-        for x, y in zip(a, b):
-            assert _same(x, y)
+    # maxiFFT::magsToDB / spectralFlatness / spectralCentroid, src/libs/maxiFFT.cpp:101-132, at three transform sizes
+    for n in (1024, 256, 2048):
+        mags = port.Stft(3, n, n // 2).process(W.channel_streams(3, 8 * n, seed=8))["mags"]
+        mags[0, 0] = 0.0                              # all-zero frame: both features return 0
+        mags[1, 1, :7] = 0.0                          # zeros are skipped by the geometric mean
+        for sr in (44100, 48000):
+            a = port.spectral_features(mags, n, sr, kind="port")
+            b = reference.spectral_features(mags, n, sr, kind="reference")
+            for x, y in zip(a, b):
+                assert _same(x, y)
 
 
 @pytest.mark.parametrize("n,hop", [(1024, 512), (1024, 256), (256, 64)])
@@ -353,7 +375,7 @@ def test_istft_bit_exact(port, reference, n, hop):
 
 # ---- maxiFFTOctaveAnalyzer / maxiBark (SURVEY.md 8f-3) ------------------------------------------------------------------------
 
-@pytest.mark.parametrize("per_octave,sr", [(1, 48000), (3, 48000), (3, 44100), (6, 48000), (0, 48000)])
+@pytest.mark.parametrize("per_octave,sr", [(1, 48000), (3, 48000), (3, 44100), (6, 48000), (0, 48000), (12, 48000)])
 def test_octave_analyser_port_equals_reference(port, reference, per_octave, sr):
     """maxiFFTOctaveAnalyzer::setup + calculate per channel (float sums in bin order, peak hold / decay carried across frames and
     calls), with the public members changed from their defaults: averages and peaks bit for bit."""
