@@ -298,6 +298,14 @@ enum {
                             owns the random stream, the stage is everything after it (lores(noise, speed, 1) * 2 sweeping two delay lines).
                             state: dl phase, dl2 phase, lopass x, lopass y; two rings (mxb_patch_get_ring returns them back to back) */
 };
+/* Operand domain: the inputs on which the reference itself is defined. Outside it the reference reads out of bounds or converts out of
+ * range, and no result is promised:
+ *   - a double -> int conversion out of range or of a NaN: a trigger, holdtime, delay size or position, flanger / chorus delay
+ *     (holdtime and the hold count are 64-bit like the reference's `long`: integral holdtimes up to 2^53 behave as there);
+ *   - the table oscillators (MXB_OSC_SINEBUF, SINEBUF4, SAWN) at a negative frequency or one above the sample rate, and SAWN at 0 Hz;
+ *   - a delay index at or beyond the ring: a size or position above delay_taps, or a negative position.
+ * Everything else -- frequencies of 0, -0, below 0, above Nyquist; duties outside [0, 1]; cutoffs, resonances and gains at and past the
+ * reference's clamps; infinities, NaNs and subnormals in any operand that is not converted to an integer -- is computed as the reference does. */
 typedef struct { int32_t op, kind, dst, reserved; int32_t src[MXB_STAGE_SRCS]; } mxb_stage;
 typedef struct {
     int32_t voices, n_stages, n_params, n_consts, n_inputs, max_frames;

@@ -82,16 +82,16 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
                 }
                 case MXB_OP_ENV_ADSR:
                 case MXB_OP_ENV_AR: {
-                    EnvRegs e;
-                    e.amp = st[sb]; e.output = st[sb + 1]; e.holdcount = (int)st[sb + 2]; env_unpack(e, (int)st[sb + 3]);
+                    PatchEnvRegs e;
+                    e.amp = st[sb]; e.output = st[sb + 1]; e.holdcount = (long long)st[sb + 2]; env_unpack(e, (int)st[sb + 3]);
                     const double in = fetch(g.src[0]);
                     const bool trig = (int)fetch(g.src[1]) == 1;
                     if (g.op == MXB_OP_ENV_ADSR) {
                         e.att = fetch(g.src[2]); e.dec = fetch(g.src[3]); e.sus = fetch(g.src[4]); e.rel = fetch(g.src[5]);
-                        e.holdtime = (int)(long long)fetch(g.src[6]);
+                        e.holdtime = (long long)fetch(g.src[6]);
                         y = env_tick(e, in, trig);
                     } else {
-                        e.att = fetch(g.src[2]); e.rel = fetch(g.src[3]); e.holdtime = (int)(long long)fetch(g.src[4]);
+                        e.att = fetch(g.src[2]); e.rel = fetch(g.src[3]); e.holdtime = (long long)fetch(g.src[4]);
                         e.dec = 0.0; e.sus = 0.0;
                         y = env_ar_tick(e, in, trig);
                     }

@@ -85,6 +85,16 @@ __device__ __forceinline__ double stage_osc(const int kind, double& phase, doubl
     return osc_tick<OSC_T_GENERIC>(phase, oout, inc, d0, kind, d1);
 }
 
+// maxiEnv::adsr / ar as a patch stage (env_tick / env_ar_tick of bank_kernels.cuh): holdtime and holdcount are 64-bit like the
+// reference's `long` (src/maximilian.h:915-916), because a patch reads holdtime from any operand -- a holdtime of 2^32 + 3 holds for
+// 2^32 + 3 samples, not 3. The bank's EnvRegs keeps 32-bit ints (mxb_bank_set_param refuses |holdtime| >= 2^31).
+struct PatchEnvRegs {
+    double amp, output, att, dec, sus, rel;
+    long long holdcount, holdtime;
+    int st;                    // ENV_* bits
+    int on, off;
+};
+
 // maxiTrigger::onZX, src/maximilian.h:564-585
 __device__ __forceinline__ double on_zx(double& previousValue, double& firstTrigger, const double input) {
     double isZX = 0.0;
@@ -114,7 +124,8 @@ __device__ __forceinline__ double envgen_tick(EgRegs& g, const double trigger, c
         if (cs.hold) g.state = 2;
         else {
             double val = pow(g.currentlevel, cs.curve);
-            val = fmax(fmin(val, 1.0), 0.0);                                   // maxiMap::linlin, src/maximilian.h:801-805
+            val = (1.0 < val) ? 1.0 : val;                                     // maxiMap::linlin, src/maximilian.h:801-805: std::min, then
+            val = (val < 0.0) ? 0.0 : val;                                     // std::max -- a NaN passes both, as it does there
             g.envval = ((val - 0.0) / (1.0 - 0.0) * (cs.endlevel - cs.startlevel)) + cs.startlevel;
             g.counter++;
             if (g.counter == cs.length) { g.counter = 0; g.currentlevel = 0; g.phase++; }

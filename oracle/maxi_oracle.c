@@ -746,7 +746,8 @@ static double p_envgen(const patch_t* p, double* st, size_t V, double trigger) {
         if (cs->hold) state = 2;
         else {
             double val = pow(currentlevel, cs->curve);
-            val = fmax(fmin(val, 1.0), 0.0);                         /* maxiMap::linlin, src/maximilian.h:801-805 */
+            val = (1.0 < val) ? 1.0 : val;                           /* maxiMap::linlin, src/maximilian.h:801-805: std::min, then */
+            val = (val < 0.0) ? 0.0 : val;                           /* std::max -- a NaN passes both, as it does there */
             envval = ((val - 0.0) / (1.0 - 0.0) * (cs->endlevel - cs->startlevel)) + cs->startlevel;
             counter++;
             if (counter == cs->length) { counter = 0; currentlevel = 0; phase++; }
