@@ -25,12 +25,6 @@ using namespace mxb;
 
 namespace {
 
-// state / register file of one thread in shared memory: slot-major, thread-minor
-struct Lane {
-    double* base; int stride;
-    __device__ __forceinline__ double& operator[](int slot) const { return base[slot * stride]; }
-};
-
 // MULTI_EG: the patch plays more than one maxiEnvGen shape. With one shape every ENVGEN stage plays shape 0, whose table and flags are then
 // read at fixed offsets of the argument block: a shape index read at run time makes ptxas spill in the stage loop, which cost the interpreter
 // about 2 % on the polysynth patch (H100 80GB HBM3, 700 W), a patch without any maxiEnvGen stage.
@@ -75,83 +69,77 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
             double y = 0.0;
             switch (g.op) {
                 case MXB_OP_OSC: {
-                    double phase = st[sb], oout = st[sb + 1];
-                    y = stage_osc(g.kind, phase, oout, fetch(g.src[0]), fetch(g.src[1]), fetch(g.src[2]), sr, a.sine, a.transition, a.sine_before);
-                    st[sb] = phase; st[sb + 1] = oout;
+                    OscRegs o; osc_state<true>(st, sb, o);
+                    y = stage_osc(g.kind, o.phase, o.output, fetch(g.src[0]), fetch(g.src[1]), fetch(g.src[2]), sr, a.sine, a.transition, a.sine_before);
+                    osc_state<false>(st, sb, o);
                     break;
                 }
                 case MXB_OP_ENV_ADSR:
                 case MXB_OP_ENV_AR: {
-                    PatchEnvRegs e;
-                    e.amp = st[sb]; e.output = st[sb + 1]; e.holdcount = (long long)st[sb + 2]; env_unpack(e, (int)st[sb + 3]);
+                    PatchEnvRegs e; env_state<true>(st, sb, e);
                     const double in = fetch(g.src[0]);
-                    const bool trig = (int)fetch(g.src[1]) == 1;
+                    const bool trig = trigger_arg(fetch(g.src[1]));
                     if (g.op == MXB_OP_ENV_ADSR) {
                         e.att = fetch(g.src[2]); e.dec = fetch(g.src[3]); e.sus = fetch(g.src[4]); e.rel = fetch(g.src[5]);
-                        e.holdtime = (long long)fetch(g.src[6]);
+                        e.holdtime = env_holdtime<PatchEnvRegs>(fetch(g.src[6]));
                         y = env_tick(e, in, trig);
                     } else {
-                        e.att = fetch(g.src[2]); e.rel = fetch(g.src[3]); e.holdtime = (long long)fetch(g.src[4]);
+                        e.att = fetch(g.src[2]); e.rel = fetch(g.src[3]); e.holdtime = env_holdtime<PatchEnvRegs>(fetch(g.src[4]));
                         e.dec = 0.0; e.sus = 0.0;
                         y = env_ar_tick(e, in, trig);
                     }
-                    st[sb] = e.amp; st[sb + 1] = e.output; st[sb + 2] = (double)e.holdcount; st[sb + 3] = (double)env_pack(e);
+                    env_state<false>(st, sb, e);
                     break;
                 }
                 case MXB_OP_ENVGEN: {
-                    // slots: 0 envval, 1 phase, 2 state, 3 nxcHappened, 4 counter, 5 currentlevel, 6/7 trigDetector, 8/9 holdDetector,
-                    // 10/11 retriggerDetector (previousValue, firstTrigger)
-                    EgRegs q;
-                    q.envval = st[sb]; q.phase = (int)st[sb + 1]; q.state = (int)st[sb + 2]; q.nxc = st[sb + 3] != 0.0;
-                    q.counter = (long long)st[sb + 4]; q.currentlevel = st[sb + 5];
-                    q.tp = st[sb + 6]; q.tf = st[sb + 7]; q.hp = st[sb + 8]; q.hf = st[sb + 9]; q.rp = st[sb + 10]; q.rf = st[sb + 11];
+                    EgRegs q; envgen_state<true>(st, sb, q);
                     const int k = MULTI_EG ? g.kind : 0;
                     y = envgen_tick(q, fetch(g.src[0]), a.eg[k], a.eg_n[k], a.eg_loop[k], a.eg_retrigger[k]);
-                    st[sb] = q.envval; st[sb + 1] = (double)q.phase; st[sb + 2] = (double)q.state; st[sb + 3] = q.nxc ? 1.0 : 0.0;
-                    st[sb + 4] = (double)q.counter; st[sb + 5] = q.currentlevel;
-                    st[sb + 6] = q.tp; st[sb + 7] = q.tf; st[sb + 8] = q.hp; st[sb + 9] = q.hf; st[sb + 10] = q.rp; st[sb + 11] = q.rf;
+                    envgen_state<false>(st, sb, q);
                     break;
                 }
                 case MXB_OP_FILTER: {
                     const double in = fetch(g.src[0]);
+                    FiltRegs f;
                     if (g.kind == MXB_FILT_LORES || g.kind == MXB_FILT_HIRES) {
-                        FiltRegs f; f.s0 = st[sb]; f.s1 = st[sb + 1];
+                        filt_state<2, true>(st, sb, f);
                         filt_design<FILT_T_LORES>(f, fetch(g.src[1]), fetch(g.src[2]), sr);
                         y = g.kind == MXB_FILT_LORES ? filt_tick<FILT_T_LORES>(f, in, nullptr) : filt_tick<FILT_T_HIRES>(f, in, nullptr);
-                        st[sb] = f.s0; st[sb + 1] = f.s1;
+                        filt_state<2, false>(st, sb, f);
                     } else if (g.kind == MXB_FILT_LOPASS || g.kind == MXB_FILT_HIPASS) {
-                        double z0 = st[sb];
-                        y = onepole_tick(g.kind, z0, in, fetch(g.src[1]));
-                        st[sb] = z0;
+                        filt_state<1, true>(st, sb, f);
+                        y = onepole_tick(g.kind, f.s0, in, fetch(g.src[1]));
+                        filt_state<1, false>(st, sb, f);
                     } else {
-                        double c0, c1, c2, z0 = st[sb], z1 = st[sb + 1];
+                        filt_state<2, true>(st, sb, f);
+                        double c0, c1, c2;
                         design_bandpass(fetch(g.src[1]), fetch(g.src[2]), sr, c0, c1, c2);
-                        y = bandpass_tick(z0, z1, in, c0, c1, c2);
-                        st[sb] = z0; st[sb + 1] = z1;
+                        y = bandpass_tick(f.s0, f.s1, in, c0, c1, c2);
+                        filt_state<2, false>(st, sb, f);
                     }
                     break;
                 }
                 case MXB_OP_SVF: {
-                    FiltRegs f; f.s0 = st[sb]; f.s1 = st[sb + 1]; f.s2 = st[sb + 2];
+                    FiltRegs f; filt_state<3, true>(st, sb, f);
                     filt_design<FILT_T_SVF>(f, fetch(g.src[1]), fetch(g.src[2]), sr);
                     const double mixw[4] = {fetch(g.src[3]), fetch(g.src[4]), fetch(g.src[5]), fetch(g.src[6])};
                     y = filt_tick<FILT_T_SVF>(f, fetch(g.src[0]), mixw);
-                    st[sb] = f.s0; st[sb + 1] = f.s1; st[sb + 2] = f.s2;
+                    filt_state<3, false>(st, sb, f);
                     break;
                 }
                 case MXB_OP_BIQUAD: {
-                    FiltRegs f; f.s0 = st[sb]; f.s1 = st[sb + 1];
+                    FiltRegs f; filt_state<2, true>(st, sb, f);
                     double cf[5];
                     design_biquad_one(g.kind, fetch(g.src[1]), fetch(g.src[2]), fetch(g.src[3]), sr, cf);
                     f.c0 = cf[0]; f.c1 = cf[1]; f.c2 = cf[2]; f.c3 = cf[3]; f.c4 = cf[4];
                     y = filt_tick<FILT_T_BIQUAD>(f, fetch(g.src[0]), nullptr);
-                    st[sb] = f.s0; st[sb + 1] = f.s1;
+                    filt_state<2, false>(st, sb, f);
                     break;
                 }
                 case MXB_OP_DCBLOCK: {
-                    double xm1 = st[sb], ym1 = st[sb + 1];
-                    y = dcblock_tick(xm1, ym1, fetch(g.src[0]), fetch(g.src[1]));
-                    st[sb] = xm1; st[sb + 1] = ym1;
+                    FiltRegs f; filt_state<2, true>(st, sb, f);
+                    y = dcblock_tick(f.s0, f.s1, fetch(g.src[0]), fetch(g.src[1]));
+                    filt_state<2, false>(st, sb, f);
                     break;
                 }
                 case MXB_OP_NONLIN: y = nonlin_eval(g.kind, fetch(g.src[0]), fetch(g.src[1]), fetch(g.src[2])); break;
@@ -159,30 +147,30 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
                 case MXB_OP_FLANGER: {
                     double* ring = a.rings + (size_t)s_ring[si] * (size_t)a.taps * V + vv;      // slot r of this voice at ring[r * V]
                     const double in = fetch(g.src[0]);
-                    int ph = (int)st[sb];
+                    int ph; delay_state<true>(st, sb, ph);
                     if (g.op == MXB_OP_DELAY) {
-                        const int size = (int)fetch(g.src[1]);
+                        const int size = int_arg(fetch(g.src[1]));
                         const double fb = fetch(g.src[2]);
                         const bool fp = g.kind == MXB_DELAY_FROM_POSITION;
-                        y = delay_tick(fp, ring, V, a.taps, live, ph, in, size, fb, fp ? (int)fetch(g.src[3]) : 0);
+                        y = delay_tick(fp, ring, V, a.taps, live, ph, in, size, fb, fp ? int_arg(fetch(g.src[3])) : 0);
                     } else {
-                        double lph = st[sb + 1], lout = st[sb + 2];
-                        const unsigned int delay = (unsigned int)fetch(g.src[1]);
+                        OscRegs lfo; osc_state<true>(st, sb + 1, lfo);
+                        const unsigned int delay = uint_arg(fetch(g.src[1]));
                         const double fb = fetch(g.src[2]);
-                        y = flanger_tick(ring, V, a.taps, live, ph, lph, lout, in, delay, fb, fetch(g.src[3]), fetch(g.src[4]), sr);
-                        st[sb + 1] = lph; st[sb + 2] = lout;
+                        y = flanger_tick(ring, V, a.taps, live, ph, lfo.phase, lfo.output, in, delay, fb, fetch(g.src[3]), fetch(g.src[4]), sr);
+                        osc_state<false>(st, sb + 1, lfo);
                     }
-                    st[sb] = (double)ph;
+                    delay_state<false>(st, sb, ph);
                     break;
                 }
                 case MXB_OP_CHORUS: {
                     double* ring = a.rings + (size_t)s_ring[si] * (size_t)a.taps * V + vv;      // this voice's two lines: ring index s_ring[si], + 1
-                    int ph1 = (int)st[sb], ph2 = (int)st[sb + 1];
-                    FiltRegs lp; lp.s0 = st[sb + 2]; lp.s1 = st[sb + 3];
+                    int ph1, ph2;
+                    FiltRegs lp; chorus_state<true>(st, sb, ph1, ph2, lp);
                     filt_design<FILT_T_LORES>(lp, fetch(g.src[3]), 1.0, sr);
-                    y = chorus_tick(ring, ring + (size_t)a.taps * V, V, a.taps, live, ph1, ph2, lp, fetch(g.src[0]), (unsigned int)fetch(g.src[1]), fetch(g.src[2]),
+                    y = chorus_tick(ring, ring + (size_t)a.taps * V, V, a.taps, live, ph1, ph2, lp, fetch(g.src[0]), uint_arg(fetch(g.src[1])), fetch(g.src[2]),
                                     fetch(g.src[4]), fetch(g.src[5]));
-                    st[sb] = (double)ph1; st[sb + 1] = (double)ph2; st[sb + 2] = lp.s0; st[sb + 3] = lp.s1;
+                    chorus_state<false>(st, sb, ph1, ph2, lp);
                     break;
                 }
                 case MXB_OP_ADD: y = fetch(g.src[0]) + fetch(g.src[1]); break;
@@ -206,8 +194,6 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
     if (live) for (int i = 0; i < a.n_state; ++i) a.state[(size_t)i * V + (size_t)v] = st[i];
 }
 
-int state_slots(const mxb_stage& g) { return patch_state_slots(g.op); }
-
 // MXB_PATCH_MODE=interpret | fused overrides the default (fused) for patches created afterwards: an A/B and debugging hook
 int patch_default_mode() {
     const char* e = getenv("MXB_PATCH_MODE");
@@ -226,6 +212,30 @@ bool src_ok(int s, const mxb_patch_desc* d) {
         case 3: return k < d->n_inputs;
         default: return false;
     }
+}
+
+// The checks of a stage list that need nothing but the descriptor, shared by mxb_patch_create / create2 and mxb_patch_codegen: a program
+// the code generator accepts is one a patch can be created from. ENVGEN kinds index the first `n_shapes` maxiEnvGen shapes.
+int validate_stages(const mxb_patch_desc* d, const int n_shapes, const char* who) {
+    MXB_REQUIRE(d->n_stages > 0 && d->n_stages <= kMaxStages, MXB_ERR_INVALID, "%s: n_stages %d (1..%d)", who, d->n_stages, kMaxStages);
+    MXB_REQUIRE(d->n_params >= 0 && d->n_params <= kMaxParams && d->n_consts >= 0 && d->n_consts <= kMaxConsts && d->n_inputs >= 0 && d->n_inputs <= kMaxInputs,
+                MXB_ERR_INVALID, "%s: n_params %d n_consts %d n_inputs %d", who, d->n_params, d->n_consts, d->n_inputs);
+    MXB_REQUIRE(d->n_consts == 0 || d->consts, MXB_ERR_INVALID, "%s: consts is NULL", who);
+    for (int i = 0; d->input_types && i < d->n_inputs; ++i)
+        MXB_REQUIRE(d->input_types[i] >= MXB_IN_F64 && d->input_types[i] <= MXB_IN_BITS, MXB_ERR_INVALID, "%s: input_types[%d] = %d", who, i, d->input_types[i]);
+    for (int i = 0; i < d->n_stages; ++i) {
+        const mxb_stage& g = d->stages[i];
+        MXB_REQUIRE(g.op >= MXB_OP_OSC && g.op <= MXB_OP_CHORUS, MXB_ERR_INVALID, "%s: stage %d: unknown op %d", who, i, g.op);
+        MXB_REQUIRE(g.dst == MXB_NONE || (g.dst >= 0 && g.dst < kMaxRegs), MXB_ERR_INVALID, "%s: stage %d: dst %d", who, i, g.dst);
+        for (int k = 0; k < MXB_STAGE_SRCS; ++k) MXB_REQUIRE(src_ok(g.src[k], d), MXB_ERR_INVALID, "%s: stage %d: operand %d = 0x%x", who, i, k, g.src[k]);
+        if (g.op == MXB_OP_OSC) MXB_REQUIRE(g.kind >= MXB_OSC_SINEWAVE && g.kind <= MXB_OSC_SAWN, MXB_ERR_INVALID, "%s: stage %d: osc kind %d", who, i, g.kind);
+        if (g.op == MXB_OP_FILTER) MXB_REQUIRE(g.kind == MXB_FILT_LORES || g.kind == MXB_FILT_HIRES || g.kind == MXB_FILT_LOPASS || g.kind == MXB_FILT_HIPASS || g.kind == MXB_FILT_BANDPASS,
+                                               MXB_ERR_INVALID, "%s: stage %d: filter kind %d", who, i, g.kind);
+        if (g.op == MXB_OP_BIQUAD) MXB_REQUIRE(g.kind >= MXB_BQ_LOWPASS && g.kind <= MXB_BQ_HIGHSHELF, MXB_ERR_INVALID, "%s: stage %d: biquad type %d", who, i, g.kind);
+        if (g.op == MXB_OP_NONLIN) MXB_REQUIRE(g.kind >= MXB_NL_ATANDIST && g.kind <= MXB_NL_FASTATAN, MXB_ERR_INVALID, "%s: stage %d: nonlinearity %d", who, i, g.kind);
+        if (g.op == MXB_OP_ENVGEN) MXB_REQUIRE(g.kind >= 0 && g.kind < n_shapes, MXB_ERR_INVALID, "%s: stage %d: envelope shape %d of %d", who, i, g.kind, n_shapes);
+    }
+    return MXB_OK;
 }
 
 // maxiEnvGen::setup + setupSegmentTime, src/maximilian.h:2371-2402, 2524-2538: the segment table of one shape from levels / times / curves
@@ -251,10 +261,6 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
     MXB_REQUIRE(ctx && d && out && d->stages, MXB_ERR_INVALID, "%s: NULL argument", who);
     *out = nullptr;
     MXB_REQUIRE(d->voices > 0 && d->max_frames > 0, MXB_ERR_INVALID, "%s: voices %d max_frames %d", who, d->voices, d->max_frames);
-    MXB_REQUIRE(d->n_stages > 0 && d->n_stages <= kMaxStages, MXB_ERR_INVALID, "%s: n_stages %d (1..%d)", who, d->n_stages, kMaxStages);
-    MXB_REQUIRE(d->n_params >= 0 && d->n_params <= kMaxParams && d->n_consts >= 0 && d->n_consts <= kMaxConsts && d->n_inputs >= 0 && d->n_inputs <= kMaxInputs,
-                MXB_ERR_INVALID, "%s: n_params %d n_consts %d n_inputs %d", who, d->n_params, d->n_consts, d->n_inputs);
-    MXB_REQUIRE(d->n_consts == 0 || d->consts, MXB_ERR_INVALID, "%s: consts is NULL", who);
     MXB_REQUIRE(d->delay_taps >= 0, MXB_ERR_INVALID, "%s: delay_taps %d", who, d->delay_taps);
     MXB_REQUIRE(n_shapes >= 0 && n_shapes <= kMaxEgShapes, MXB_ERR_INVALID, "%s: n_shapes %d (0..%d)", who, n_shapes, kMaxEgShapes);
     MXB_REQUIRE(n_shapes == 0 || shapes, MXB_ERR_INVALID, "%s: shapes is NULL", who);
@@ -266,26 +272,15 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
         for (int i = 0; i < s.stages; ++i) holds += s.times[i] == MXB_ENVGEN_HOLD;
         MXB_REQUIRE(holds <= 1, MXB_ERR_INVALID, "%s: shape %d has %d HOLD segments (maxiEnvGen::setup allows one)", who, k, holds);
     }
-    for (int i = 0; d->input_types && i < d->n_inputs; ++i)
-        MXB_REQUIRE(d->input_types[i] >= MXB_IN_F64 && d->input_types[i] <= MXB_IN_BITS, MXB_ERR_INVALID, "%s: input_types[%d] = %d", who, i, d->input_types[i]);
+    int rc = validate_stages(d, n_shapes, who);
+    if (rc != MXB_OK) return rc;
     int n_state = 0, n_rings = 0;
     bool tables = false;
     for (int i = 0; i < d->n_stages; ++i) {
         const mxb_stage& g = d->stages[i];
-        MXB_REQUIRE(g.op >= MXB_OP_OSC && g.op <= MXB_OP_CHORUS, MXB_ERR_INVALID, "%s: stage %d: unknown op %d", who, i, g.op);
-        MXB_REQUIRE(g.dst == MXB_NONE || (g.dst >= 0 && g.dst < kMaxRegs), MXB_ERR_INVALID, "%s: stage %d: dst %d", who, i, g.dst);
-        for (int k = 0; k < MXB_STAGE_SRCS; ++k) MXB_REQUIRE(src_ok(g.src[k], d), MXB_ERR_INVALID, "%s: stage %d: operand %d = 0x%x", who, i, k, g.src[k]);
-        if (g.op == MXB_OP_OSC) {
-            MXB_REQUIRE(g.kind >= MXB_OSC_SINEWAVE && g.kind <= MXB_OSC_SAWN, MXB_ERR_INVALID, "%s: stage %d: osc kind %d", who, i, g.kind);
-            tables = tables || g.kind >= MXB_OSC_SINEBUF;
-        }
-        if (g.op == MXB_OP_FILTER) MXB_REQUIRE(g.kind == MXB_FILT_LORES || g.kind == MXB_FILT_HIRES || g.kind == MXB_FILT_LOPASS || g.kind == MXB_FILT_HIPASS || g.kind == MXB_FILT_BANDPASS,
-                                               MXB_ERR_INVALID, "%s: stage %d: filter kind %d", who, i, g.kind);
-        if (g.op == MXB_OP_BIQUAD) MXB_REQUIRE(g.kind >= MXB_BQ_LOWPASS && g.kind <= MXB_BQ_HIGHSHELF, MXB_ERR_INVALID, "%s: stage %d: biquad type %d", who, i, g.kind);
-        if (g.op == MXB_OP_NONLIN) MXB_REQUIRE(g.kind >= MXB_NL_ATANDIST && g.kind <= MXB_NL_FASTATAN, MXB_ERR_INVALID, "%s: stage %d: nonlinearity %d", who, i, g.kind);
-        if (g.op == MXB_OP_ENVGEN) MXB_REQUIRE(g.kind >= 0 && g.kind < n_shapes, MXB_ERR_INVALID, "%s: stage %d: envelope shape %d of %d", who, i, g.kind, n_shapes);
+        tables = tables || (g.op == MXB_OP_OSC && g.kind >= MXB_OSC_SINEBUF);
         if (patch_stage_rings(g.op)) { MXB_REQUIRE(d->delay_taps > 0, MXB_ERR_INVALID, "%s: stage %d needs delay_taps > 0", who, i); n_rings += patch_stage_rings(g.op); }
-        n_state += state_slots(g);
+        n_state += patch_state_slots(g.op);
     }
     if (tables) MXB_REQUIRE(ctx->d_sine, MXB_ERR_STATE, "%s: sinebuf / sinebuf4 / sawn need the reference's tables: call mxb_ctx_set_tables first", who);
     const size_t per_thread = (size_t)(kMaxRegs + d->n_params + n_state);
@@ -301,7 +296,7 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
     for (int i = 0; i < d->n_inputs; ++i) p->in_type[i] = d->input_types ? d->input_types[i] : MXB_IN_F64;
     int sb = 0, ri = 0;
     for (int i = 0; i < d->n_stages; ++i) {
-        p->state_base.push_back(sb); sb += state_slots(p->stages[i]);
+        p->state_base.push_back(sb); sb += patch_state_slots(p->stages[i].op);
         const int nr = patch_stage_rings(p->stages[i].op);
         p->ring_of.push_back(nr ? ri : -1);
         ri += nr;
@@ -312,7 +307,6 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
         eg_segments(shapes[k], (double)(size_t)ctx->sample_rate, p->eg[k]);
     }
     const size_t V = (size_t)p->V;
-    int rc = MXB_OK;
 #define TRY(x) do { rc = (x); if (rc != MXB_OK) { mxb_patch_destroy(p); return rc; } } while (0)
     TRY(dev_alloc(&p->d_stages, (size_t)d->n_stages)); TRY(dev_alloc(&p->d_state_base, (size_t)d->n_stages)); TRY(dev_alloc(&p->d_ring_of, (size_t)d->n_stages));
     TRY(dev_alloc(&p->d_consts, (size_t)kMaxConsts));
@@ -324,13 +318,12 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
     if (e == cudaSuccess) e = cudaMemcpy(p->d_state_base, p->state_base.data(), sizeof(int) * d->n_stages, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(p->d_ring_of, p->ring_of.data(), sizeof(int) * d->n_stages, cudaMemcpyHostToDevice);
     if (e == cudaSuccess && d->n_consts) e = cudaMemcpy(p->d_consts, d->consts, sizeof(double) * d->n_consts, cudaMemcpyHostToDevice);
-    // initial state that is not zero in the reference: maxiTrigger (previousValue = 1, firstTrigger = 1, src/maximilian.h:583-584)
-    for (int i = 0; i < d->n_stages && e == cudaSuccess; ++i) {
-        if (p->stages[i].op != MXB_OP_ENVGEN) continue;
-        std::vector<double> ones(V, 1.0);
-        for (int k = 6; k < 12 && e == cudaSuccess; ++k)
-            e = cudaMemcpy(p->state + (size_t)(p->state_base[i] + k) * V, ones.data(), sizeof(double) * V, cudaMemcpyHostToDevice);
-    }
+    for (int i = 0; i < d->n_stages && e == cudaSuccess; ++i)
+        for (int k = 0; k < patch_state_slots(p->stages[i].op) && e == cudaSuccess; ++k)
+            if (patch_state_init(p->stages[i].op, k) != 0.0) {                 // dev_alloc zeroed the others
+                const std::vector<double> col(V, patch_state_init(p->stages[i].op, k));
+                e = cudaMemcpy(p->state + (size_t)(p->state_base[i] + k) * V, col.data(), sizeof(double) * V, cudaMemcpyHostToDevice);
+            }
     if (e != cudaSuccess) { set_error("%s: %s", who, cudaGetErrorString(e)); mxb_patch_destroy(p); return MXB_ERR_CUDA; }
 #undef TRY
     *out = p;
@@ -394,7 +387,7 @@ int32_t mxb_patch_set_param(mxb_patch* p, int32_t j, const double* values, int32
 static int32_t patch_state_ptr(mxb_patch* p, int32_t stage, int32_t slot, double** ptr, const char* who) {
     MXB_REQUIRE(p, MXB_ERR_INVALID, "%s: NULL patch", who);
     MXB_REQUIRE(stage >= 0 && stage < p->n_stages, MXB_ERR_INVALID, "%s: stage %d of %d", who, stage, p->n_stages);
-    MXB_REQUIRE(slot >= 0 && slot < state_slots(p->stages[stage]), MXB_ERR_INVALID, "%s: stage %d has %d state slots, not %d", who, stage, state_slots(p->stages[stage]), slot);
+    MXB_REQUIRE(slot >= 0 && slot < patch_state_slots(p->stages[stage].op), MXB_ERR_INVALID, "%s: stage %d has %d state slots, not %d", who, stage, patch_state_slots(p->stages[stage].op), slot);
     *ptr = p->state + (size_t)(p->state_base[stage] + slot) * p->V;
     return MXB_OK;
 }
@@ -448,26 +441,15 @@ int32_t mxb_patch_get_mode(const mxb_patch* p) { return p ? p->mode : MXB_ERR_IN
 
 int32_t mxb_patch_codegen(const mxb_patch_desc* d, char* buf, int64_t cap, int64_t* needed, int32_t compile) {
     MXB_REQUIRE(d && d->stages && needed, MXB_ERR_INVALID, "mxb_patch_codegen: NULL argument");
-    MXB_REQUIRE(d->n_stages > 0 && d->n_stages <= kMaxStages && d->n_params >= 0 && d->n_params <= kMaxParams && d->n_consts >= 0 && d->n_consts <= kMaxConsts &&
-                d->n_inputs >= 0 && d->n_inputs <= kMaxInputs && (d->n_consts == 0 || d->consts), MXB_ERR_INVALID, "mxb_patch_codegen: bad descriptor");
-    for (int i = 0; i < d->n_stages; ++i) {
-        const mxb_stage& g = d->stages[i];
-        MXB_REQUIRE(g.op >= MXB_OP_OSC && g.op <= MXB_OP_CHORUS && (g.dst == MXB_NONE || (g.dst >= 0 && g.dst < kMaxRegs)), MXB_ERR_INVALID, "mxb_patch_codegen: stage %d", i);
-        for (int k = 0; k < MXB_STAGE_SRCS; ++k) MXB_REQUIRE(src_ok(g.src[k], d), MXB_ERR_INVALID, "mxb_patch_codegen: stage %d: operand %d = 0x%x", i, k, g.src[k]);
-        if (g.op == MXB_OP_ENVGEN) MXB_REQUIRE(g.kind >= 0 && g.kind < kMaxEgShapes, MXB_ERR_INVALID, "mxb_patch_codegen: stage %d: envelope shape %d (0..%d)", i, g.kind, kMaxEgShapes - 1);
-    }
-    int types[kMaxInputs] = {};
-    for (int i = 0; d->input_types && i < d->n_inputs; ++i) {
-        MXB_REQUIRE(d->input_types[i] >= MXB_IN_F64 && d->input_types[i] <= MXB_IN_BITS, MXB_ERR_INVALID, "mxb_patch_codegen: input_types[%d] = %d", i, d->input_types[i]);
-        types[i] = d->input_types[i];
-    }
-    const std::string src = patch_generate_source(d->stages, d->n_stages, d->n_params, d->consts, d->n_consts, d->n_inputs, types);
+    const int rc = validate_stages(d, kMaxEgShapes, "mxb_patch_codegen");      // the shapes are kernel arguments: any of them may be set
+    if (rc != MXB_OK) return rc;
+    const std::string src = patch_generate_source(d->stages, d->n_stages, d->n_params, d->consts, d->n_consts, d->n_inputs, d->input_types);
     *needed = (int64_t)src.size() + 1;
     if (buf && cap > 0) { const size_t n = src.size() + 1 <= (size_t)cap ? src.size() : (size_t)cap - 1; memcpy(buf, src.data(), n); buf[n] = 0; }
     if (compile) {
         std::vector<char> cubin;
-        const int rc = patch_compile(src, cubin);
-        if (rc != MXB_OK) return rc;
+        const int crc = patch_compile(src, cubin);
+        if (crc != MXB_OK) return crc;
         MXB_REQUIRE(!cubin.empty(), MXB_ERR_STATE, "mxb_patch_codegen: the compiler returned no code");
     }
     return MXB_OK;

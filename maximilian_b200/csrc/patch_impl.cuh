@@ -1,5 +1,6 @@
 // Voice patches: what the interpreting kernel (patch.cu) and the kernels generated per patch (patch_fuse.cu, compiled at
-// run time with NVRTC) share -- the argument block and the stage bodies. Each body is the reference method restated (same
+// run time with NVRTC) share -- the argument block, the stage bodies, each stage's state layout and the conversions of its
+// operands. Each body is the reference method restated (same
 // statements, same order; compiled without multiply-add contraction), taking its stage kind as a plain int: the interpreter
 // passes it at run time (warp-uniform), a generated kernel passes a literal and the branches fold away.
 //
@@ -240,22 +241,64 @@ __device__ __forceinline__ void mix_warp_store(double ml, double mr, const int l
     if ((lane & 15) == 0) partials[(t * 2 + (up ? 1 : 0)) * W + gwarp] = v;
 }
 
-// number of state words of a stage (the order documented with the ops in maxib200.h)
-__host__ __device__ inline int patch_state_slots(const int op) {
-    switch (op) {
-        case MXB_OP_OSC: return 2;
-        case MXB_OP_ENV_ADSR: case MXB_OP_ENV_AR: return 4;
-        case MXB_OP_ENVGEN: return 12;
-        case MXB_OP_FILTER: return 2;
-        case MXB_OP_SVF: return 3;
-        case MXB_OP_BIQUAD: return 2;
-        case MXB_OP_DCBLOCK: return 2;
-        case MXB_OP_DELAY: return 1;
-        case MXB_OP_FLANGER: return 3;
-        case MXB_OP_CHORUS: return 4;
-        default: return 0;
-    }
+// ---- the state layout: which of a stage's state words holds which member (maxib200.h documents the order with the ops) ----
+// One function per stateful op moves its registers in (LOAD) or out of its words over an accessor, anything with `double& operator[](int)
+// const` (by value): the interpreter's Lane over shared memory, or a generated kernel's StateColumn, where `sb` is a literal.
+// one thread's registers, parameters or state in the interpreter's shared memory: slot-major, thread-minor
+struct Lane {
+    double* base; int stride;
+    __device__ __forceinline__ double& operator[](int slot) const { return base[slot * stride]; }
+};
+// voice v's words of a.state (read from the argument block at each use: a kernel then compiles as if it indexed a.state itself)
+struct StateColumn {
+    const PatchArgs& a; size_t V; long long v;
+    __device__ __forceinline__ double& operator[](int k) const { return a.state[(size_t)k * V + (size_t)v]; }
+};
+template <bool LOAD, class T> __device__ __forceinline__ void word(double& w, T& m) { if (LOAD) m = (T)w; else w = (double)m; }     // one word, one member
+template <bool LOAD> __device__ __forceinline__ void word(double& w, bool& m) { if (LOAD) m = w != 0.0; else w = m ? 1.0 : 0.0; }
+// OSC: phase, output
+struct OscRegs { double phase, output; };
+template <bool LOAD, class A> __device__ __forceinline__ void osc_state(const A s, const int sb, OscRegs& o) { word<LOAD>(s[sb], o.phase); word<LOAD>(s[sb + 1], o.output); }
+// ENV_ADSR / ENV_AR: amp, output, holdcount, the ENV_* flags (E: PatchEnvRegs, or EnvRegs for a constant 32-bit holdtime)
+template <bool LOAD, class A, class E> __device__ __forceinline__ void env_state(const A s, const int sb, E& e) {
+    word<LOAD>(s[sb], e.amp); word<LOAD>(s[sb + 1], e.output); word<LOAD>(s[sb + 2], e.holdcount);
+    if (LOAD) env_unpack(e, (int)s[sb + 3]); else s[sb + 3] = (double)env_pack(e);
 }
+// ENVGEN: 0 envval, 1 phase, 2 state, 3 nxcHappened, 4 counter, 5 currentlevel, 6/7 trigDetector, 8/9 holdDetector,
+// 10/11 retriggerDetector (previousValue, firstTrigger)
+template <bool LOAD, class A> __device__ __forceinline__ void envgen_state(const A s, const int sb, EgRegs& q) {
+    word<LOAD>(s[sb], q.envval); word<LOAD>(s[sb + 1], q.phase); word<LOAD>(s[sb + 2], q.state); word<LOAD>(s[sb + 3], q.nxc); word<LOAD>(s[sb + 4], q.counter);
+    word<LOAD>(s[sb + 5], q.currentlevel); word<LOAD>(s[sb + 6], q.tp); word<LOAD>(s[sb + 7], q.tf); word<LOAD>(s[sb + 8], q.hp); word<LOAD>(s[sb + 9], q.hf);
+    word<LOAD>(s[sb + 10], q.rp); word<LOAD>(s[sb + 11], q.rf);
+}
+// filters: the first N words of FiltRegs' history. FILTER lores / hires, BIQUAD: s0, s1; FILTER lopass / hipass: s0; FILTER bandpass:
+// its two outputs; SVF: s0, s1, s2; DCBLOCK: xm1, ym1
+template <int N, bool LOAD, class A> __device__ __forceinline__ void filt_state(const A s, const int sb, FiltRegs& f) {
+    word<LOAD>(s[sb], f.s0);
+    if (N > 1) word<LOAD>(s[sb + 1], f.s1);
+    if (N > 2) word<LOAD>(s[sb + 2], f.s2);
+}
+// DELAY: the ring index. FLANGER: the same, then its triangle LFO's OSC words at sb + 1 (its maxiDelayline and maxiOsc)
+template <bool LOAD, class A> __device__ __forceinline__ void delay_state(const A s, const int sb, int& ph) { word<LOAD>(s[sb], ph); }
+// CHORUS: the two ring indices, then the lores LFO's s0, s1
+template <bool LOAD, class A> __device__ __forceinline__ void chorus_state(const A s, const int sb, int& ph1, int& ph2, FiltRegs& lp) {
+    word<LOAD>(s[sb], ph1); word<LOAD>(s[sb + 1], ph2); filt_state<2, LOAD>(s, sb + 2, lp);
+}
+
+// ---- operands as the reference's methods take them (every operand arrives as a double) ----
+__device__ __forceinline__ bool trigger_arg(const double x) { return (int)x == 1; }                  // maxiEnv's `int trigger`
+__device__ __forceinline__ int int_arg(const double x) { return (int)x; }                            // a delay line's size or position
+__device__ __forceinline__ unsigned int uint_arg(const double x) { return (unsigned int)x; }         // maxiFlanger / maxiChorus delay
+// maxiEnv's `long holdtime`, in the width of the register type E
+template <class E> __device__ __forceinline__ decltype(E::holdtime) env_holdtime(const double x) { return (decltype(E::holdtime))(long long)x; }
+
+// number of state words of a stage, by op: OSC 2, ENV_ADSR / ENV_AR 4, ENVGEN 12, FILTER 2, SVF 3, BIQUAD 2, DCBLOCK 2, DELAY 1, FLANGER 3, CHORUS 4
+__host__ __device__ inline int patch_state_slots(const int op) {
+    constexpr int slots[MXB_OP_CHORUS + 1] = {0, 2, 4, 4, 12, 2, 3, 2, 2, 0, 1, 3, 0, 0, 0, 0, 0, 0, 4};
+    return op >= 0 && op <= MXB_OP_CHORUS ? slots[op] : 0;
+}
+// initial value of a state word: 0, but for maxiEnvGen's maxiTrigger detectors (previousValue = 1, firstTrigger = 1, src/maximilian.h:583-584)
+__host__ __device__ inline double patch_state_init(const int op, const int slot) { return op == MXB_OP_ENVGEN && slot >= 6 ? 1.0 : 0.0; }
 // delay lines (rings of delay_taps slots) a stage owns
 __host__ __device__ inline int patch_stage_rings(const int op) { return op == MXB_OP_CHORUS ? 2 : (op == MXB_OP_DELAY || op == MXB_OP_FLANGER) ? 1 : 0; }
 

@@ -12,6 +12,9 @@ BIQUAD = dict(lowpass=0, highpass=1, bandpass=2, notch=3, peak=4, lowshelf=5, hi
 NONLIN = dict(atandist=0, fastatandist=1, softclip=2, hardclip=3, asymclip=4, fastatan=5)
 DELAY = dict(dl=0, position=1)
 KINDS = dict(osc=OSC, filter=FILT, biquad=BIQUAD, nonlin=NONLIN, delay=DELAY)
+# state words of a stage, by op (the layouts include/maxib200.h documents with the ops); ops not listed have none
+STATE_SLOTS = {OP["osc"]: 2, OP["env_adsr"]: 4, OP["env_ar"]: 4, OP["envgen"]: 12, OP["filter"]: 2, OP["svf"]: 3, OP["biquad"]: 2,
+               OP["dcblock"]: 2, OP["delay"]: 1, OP["flanger"]: 3, OP["chorus"]: 4}
 ENVGEN_HOLD = -46692.0
 NONE = -1
 NSRC = 8

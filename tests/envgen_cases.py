@@ -5,10 +5,10 @@ watches zero crossings: the positive one starts the envelope, the negative one e
 and close again inside a segment, which retriggers a shape that allows it."""
 import numpy as np
 
-from maximilian_b200.patchdef import PatchDef, R, ENVGEN_HOLD
+from maximilian_b200.patchdef import PatchDef, R, ENVGEN_HOLD, OP, STATE_SLOTS
 from maximilian_b200 import workloads as W
 
-SLOTS = 12      # state words of an ENVGEN stage (include/maxib200.h)
+SLOTS = STATE_SLOTS[OP["envgen"]]      # state words of an ENVGEN stage
 
 
 def swing(V, n, seed, density=0.02, hold=(3, 120)):

@@ -12,27 +12,12 @@ import pytest
 
 import golden_checks as G
 import patch_cases as PC
+from patch_checks import INT_SLOTS, cmp as _cmp, set_tables as _tables
 from maximilian_b200 import capi
 from maximilian_b200 import workloads as W
+from maximilian_b200.patchdef import STATE_SLOTS as SLOTS
 
 pytestmark = pytest.mark.gpu
-
-SLOTS = {1: 2, 2: 4, 3: 4, 4: 12, 5: 2, 6: 3, 7: 2, 8: 2, 10: 1, 11: 3, 18: 4}
-INT_SLOTS = {2: (2, 3), 3: (2, 3), 4: (1, 2, 4), 10: (0,), 11: (0,), 18: (0, 1)}          # integral members: exact whatever the patch
-
-
-def _tables(port):
-    g = G.load("tables")
-    port.set_tables(g["sine"], g["transition"], float(g["sine_before"]), "port")
-    capi.set_tables(g["sine"], g["transition"], float(g["sine_before"]))
-
-
-def _cmp(got, ref, exact, what):
-    if exact:
-        assert np.array_equal(got, ref, equal_nan=True), f"{what}: not bit-identical, max abs err {np.nanmax(np.abs(got - ref))}"
-    else:
-        np.testing.assert_allclose(got, ref, rtol=1e-9, atol=1e-12, err_msg=what)
-
 
 MODES = ["fused", "interpret"]
 

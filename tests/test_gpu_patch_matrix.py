@@ -9,34 +9,19 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import golden_checks as G
 import patch_matrix as PM
+from patch_checks import BAD_KINDS, INT_SLOTS, bad_kind_patch, cmp as _cmp, ring_stages as _ring_stages, set_tables
 from maximilian_b200 import capi
-from maximilian_b200.patchdef import PatchDef, R, OP, BIQUAD, ENVGEN_HOLD
+from maximilian_b200.patchdef import PatchDef, R, OP, BIQUAD, ENVGEN_HOLD, STATE_SLOTS as SLOTS
 
 pytestmark = pytest.mark.gpu
 
-SLOTS = {1: 2, 2: 4, 3: 4, 4: 12, 5: 2, 6: 3, 7: 2, 8: 2, 10: 1, 11: 3, 18: 4}
-INT_SLOTS = {2: (2, 3), 3: (2, 3), 4: (1, 2, 4), 10: (0,), 11: (0,), 18: (0, 1)}
 MODES = ["fused", "interpret"]
 
 
 @pytest.fixture(autouse=True)
 def _tables(port):
-    g = G.load("tables")
-    port.set_tables(g["sine"], g["transition"], float(g["sine_before"]), "port")
-    capi.set_tables(g["sine"], g["transition"], float(g["sine_before"]))
-
-
-def _cmp(got, ref, exact, what):
-    if exact:
-        assert np.array_equal(got, ref, equal_nan=True), f"{what}: not bit-identical, max abs err {np.nanmax(np.abs(got - ref))}"
-    else:
-        np.testing.assert_allclose(got, ref, rtol=1e-9, atol=1e-12, err_msg=what)
-
-
-def _ring_stages(d):
-    return [(si, 2 if op == OP["chorus"] else 1) for si, (op, *_) in enumerate(d.stages) if op in (OP["delay"], OP["flanger"], OP["chorus"])]
+    set_tables(port)
 
 
 def _state(p, d, taps, voices):
@@ -486,3 +471,24 @@ def test_set_state_resumes_a_patch_mid_stream(mode):
         oa, ma = a.process(B, ins, want_mix=True); oc, mc = c.process(B, ins, want_mix=True)
         assert np.array_equal(oa, oc) and np.array_equal(ma, mc), blk
     _same_state(_state(a, d, 0, ()), _state(c, d, 0, ()), "resumed")
+
+
+def test_state_slots_table_is_the_librarys():
+    """patchdef.STATE_SLOTS against mxb_patch_get_state: a stage has exactly that many state words, every op of the matrix"""
+    seen = set()
+    for name, d, params, inputs, exact, taps in PM.cases():
+        p = capi.Patch(d, 40, max_frames=8, delay_taps=taps, mode="interpret")
+        for si, (op, *_) in enumerate(d.stages):
+            n = SLOTS.get(op, 0)
+            with pytest.raises(capi.MxbError):
+                p.get_state(si, n)
+            if n:
+                assert p.get_state(si, n - 1).shape == (40,)
+            seen.add(op)
+    assert seen == set(OP.values())
+
+
+def test_patch_create_refuses_the_kinds_the_generator_refuses():
+    for op, kind in BAD_KINDS:
+        with pytest.raises(capi.MxbError):
+            capi.Patch(bad_kind_patch(op, kind), 40, max_frames=8, mode="interpret")

@@ -9,6 +9,7 @@ import golden_checks as G
 import envgen_cases as EC
 import envgen_oracle as EO
 import patch_cases as PC
+from maximilian_b200.patchdef import STATE_SLOTS
 
 
 @pytest.mark.parametrize("case", EC.cases(), ids=lambda c: c[0])
@@ -52,7 +53,6 @@ def test_lock_step_composition_equals_the_direct_run(port):
         x = inputs(V, B, blk, 9)
         oa, ma = a.process(B, x, want_mix=True); ob, mb = b.process(B, x, want_mix=True)
         assert np.array_equal(oa, ob) and np.array_equal(ma, mb), blk
-    slots = {4: 12, 1: 2, 10: 1, 11: 3, 3: 4}
     for si, st in enumerate(d.stages):
-        for sl in range(slots.get(st[0], 0)):
+        for sl in range(STATE_SLOTS.get(st[0], 0)):
             assert np.array_equal(a.get_state(si, sl), b.get_state(si, sl)), (si, sl)

@@ -7,14 +7,8 @@ import pytest
 import golden_checks as G
 from oracle.replay import same
 import patch_cases as PC
-
-SLOTS = {1: 2, 2: 4, 3: 4, 4: 12, 5: 2, 6: 3, 7: 2, 8: 2, 10: 1, 11: 3}      # state slots per op (include/maxib200.h)
-
-
-def _tables(port):
-    g = G.load("tables")
-    port.set_tables(g["sine"], g["transition"], float(g["sine_before"]), "port")
-    return g
+from patch_checks import set_tables
+from maximilian_b200.patchdef import STATE_SLOTS as SLOTS
 
 
 def test_tables_fixture_is_the_references(port, reference):
@@ -27,7 +21,7 @@ def test_tables_fixture_is_the_references(port, reference):
 @pytest.mark.parametrize("case", PC.cases(), ids=lambda c: c[0])
 def test_patch_port_equals_reference(port, reference, case):
     name, d, params, inputs, exact, taps = case
-    _tables(port)
+    set_tables(port, library=False)
     V, B = 24, 200
     po = port.Patch(d, V, delay_taps=taps, kind="port"); pr = reference.Patch(d, V, delay_taps=taps, kind="reference")
     for k, v in params(V, 11).items():
@@ -54,7 +48,7 @@ def test_patch_port_equals_reference(port, reference, case):
 def test_patch_golden_exact(port, case):
     """tests/golden/patches.npz (made by the compiled reference) replayed through the C port: exact, wherever gcc runs."""
     name, d, params, inputs, exact, taps = case
-    _tables(port)
+    set_tables(port, library=False)
     g = G.load("patches")
     V, B, NB = int(g["V"]), int(g["B"]), int(g["NB"])
     p = port.Patch(d, V, delay_taps=taps, kind="port")

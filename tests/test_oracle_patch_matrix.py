@@ -8,13 +8,11 @@ import struct
 import numpy as np
 import pytest
 
-import golden_checks as G
 import patch_matrix as PM
+from patch_checks import set_tables
 from maximilian_b200 import capi
-from maximilian_b200.patchdef import OP, FILT, KINDS
+from maximilian_b200.patchdef import OP, FILT, KINDS, STATE_SLOTS as SLOTS
 from oracle.replay import same
-
-SLOTS = {1: 2, 2: 4, 3: 4, 4: 12, 5: 2, 6: 3, 7: 2, 8: 2, 10: 1, 11: 3, 18: 4}
 CASES = PM.cases()
 
 
@@ -35,8 +33,7 @@ def test_matrix_covers_every_op_and_kind():
 @pytest.mark.parametrize("case", CASES, ids=_ids)
 def test_matrix_port_equals_reference(port, reference, case):
     name, d, params, inputs, exact, taps = case
-    g = G.load("tables")
-    port.set_tables(g["sine"], g["transition"], float(g["sine_before"]), "port")
+    set_tables(port, library=False)
     V, B, NB, seed = 24, 200, 3, 7
     ins = [inputs(V, B, blk, seed) for blk in range(NB)]          # before srand: the port's noise_fill re-seeds libc's rand() as well
     po = port.Patch(d, V, delay_taps=taps, kind="port"); pr = reference.Patch(d, V, delay_taps=taps, kind="reference")
@@ -130,3 +127,18 @@ def test_matrix_uses_every_operand_class_and_every_special_constant():
     # every input element type feeds a trigger
     types = {d.input_types.get(n, "f64") for _, d, *_ in CASES for n in d.inputs}
     assert types == {"f64", "u8", "bits"}
+
+
+def test_state_slots_table_is_the_ports(port):
+    """patchdef.STATE_SLOTS against the C port: a stage has exactly that many state words, every op of the matrix"""
+    seen = set()
+    for name, d, params, inputs, exact, taps in CASES:
+        p = port.Patch(d, 4, delay_taps=taps, kind="port")
+        for si, (op, *_) in enumerate(d.stages):
+            n = SLOTS.get(op, 0)
+            with pytest.raises(RuntimeError):
+                p.get_state(si, n)
+            if n:
+                assert p.get_state(si, n - 1).shape == (4,)
+            seen.add(op)
+    assert seen == set(OP.values())

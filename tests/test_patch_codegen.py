@@ -9,6 +9,7 @@ import pytest
 import patch_cases as PC
 from maximilian_b200 import capi
 from maximilian_b200.patchdef import PatchDef, R
+from patch_checks import BAD_KINDS, bad_kind_patch
 
 
 @pytest.mark.parametrize("case", PC.cases() + [PC.chorus(False), PC.chorus(True)], ids=lambda c: c[0])
@@ -75,3 +76,11 @@ def test_a_program_the_generator_rejects_is_an_error_not_a_crash():
     d = PatchDef(); d.stage("add", 0x100 + 5, 0x200 + 7, dst=R(0))                 # parameter / constant that do not exist
     with pytest.raises(capi.MxbError):
         capi.patch_codegen(d)
+
+
+@pytest.mark.parametrize("op,kind", BAD_KINDS)
+def test_the_generator_refuses_what_patch_create_refuses(op, kind):
+    with pytest.raises(capi.MxbError):
+        capi.patch_codegen(bad_kind_patch(op, kind))
+    ok = bad_kind_patch(op, 0 if op != "filter" else 1)
+    assert "mxb_fused_patch" in capi.patch_codegen(ok)
