@@ -428,7 +428,8 @@ int32_t mxb_stft_process2(mxb_stft* st, const float* in, int64_t stride_c, int64
  * octave_averages / octave_peaks: float [channels][max_frames][mxb_octave_n_averages()] after each frame's calculate().
  * bark != 0: maxiBarkScaleAnalyser::setup(sample rate of the context, fft_size); bark_specific / bark_relative: double
  * [channels][max_frames][24] (specificLoudness / relativeLoudness of the magnitudes), bark_total: double [channels][max_frames].
- * pow(sum, 0.23) is libdevice's: 1e-12 relative. Built into the 1024-point kernel; other sizes: MXB_ERR_UNSUPPORTED. */
+ * pow(sum, 0.23) is libdevice's: 1e-12 relative. Fused into the 1024-point kernel only (other sizes: MXB_ERR_UNSUPPORTED); on any
+ * spectrum, at any size, mxb_octave_process / mxb_bark_process below compute the same values from magnitudes in memory. */
 typedef struct mxb_octave mxb_octave;
 int32_t mxb_octave_create(mxb_ctx* ctx, int32_t channels, float sampling_rate, int32_t n_bands, int32_t n_per_octave, mxb_octave** o);
 int32_t mxb_octave_destroy(mxb_octave* o);
@@ -441,6 +442,24 @@ typedef struct {
 int32_t mxb_stft_process3(mxb_stft* st, const float* in, int64_t stride_c, int64_t stride_t, int32_t n_samples,
                           int32_t max_frames, const mxb_stft_outputs* out, const mxb_stft_post* post, mxb_mfcc* mfcc,
                           int32_t* n_frames, int32_t mem, void* stream);
+/* maxiFFTOctaveAnalyzer::calculate(fftData) (src/libs/maxiFFT.cpp:261-300) on caller-supplied spectra, for every channel of o.
+ * mags: float, frame f of channel c at ((c*max_frames)+f)*n_bands (the layout mxb_stft_process writes), frames 0..frames-1 analysed in
+ * order. averages / peaks (each optional): float at ((c*max_frames)+f)*n_averages. The state is the handle's own: averages, peaks and
+ * hold counters, the same state the fused 1024-point epilogue carries. So one handle may alternate between the two paths.
+ * Spectra may hold NaN, inf or negative values: they flow through the float sums and the >= peak test as in the reference.
+ * frames == 0 does nothing; frames < 0 or > max_frames: MXB_ERR_INVALID. */
+int32_t mxb_octave_process(mxb_octave* o, const float* mags, int32_t frames, int32_t max_frames,
+                           float* averages, float* peaks, int32_t mem, void* stream);
+/* maxiBarkScaleAnalyser::setup(sR, bS) + specificLoudness / relativeLoudness / totalLoudness (src/libs/maxiBark.h:36-113).
+ * buffer_size: 2 .. 4096 (the reference's barkScale[2048]); sample_rate: > 0, with (buffer_size/2 - 1) * sample_rate < 2^32 (the
+ * reference's bin-to-Hz conversion is unsigned int arithmetic). The band limits do not depend on the context's sample rate. */
+typedef struct mxb_bark mxb_bark;
+int32_t mxb_bark_create(mxb_ctx* ctx, int32_t sample_rate, int32_t buffer_size, mxb_bark** b);
+int32_t mxb_bark_destroy(mxb_bark* b);
+/* spectrum: float [n][buffer_size/2]; specific / relative: double [n][24]; total: double [n] (each optional). n == 0 does nothing.
+ * NaN, inf and negative bins follow the reference through the band sum, pow and the > max scan (relative = specific / max). */
+int32_t mxb_bark_process(mxb_bark* b, const float* spectrum, int64_t n, double* specific, double* relative, double* total,
+                         int32_t mem, void* stream);
 
 /* maxiMFCC::setup(numBins, numFilters, numCoeffs, minFreq, maxFreq) + mfcc() (src/libs/maxiMFCC.h:56-111,
  * src/libs/maxiMFCC.cpp:48-66). mags: float [n][num_bins]; coeffs: double [n][num_coeffs];

@@ -706,13 +706,19 @@ private:
 
 class maxiFFT;
 
-/* maxiFFTOctaveAnalyzer, src/libs/maxiFFT.h:162-205, maxiFFT.cpp:201-300. Here calculate() is an epilogue of the transform: the analyser is
- * attached to a maxiFFT (fft.attach(oct), before or after setup()), whose process() then runs it for every frame it fires, on the device,
- * while the magnitudes are on chip. The public members keep the reference's names: peakHoldTime, peakDecayRate, linearEQIntercept and
- * linearEQSlope are read at every process(); `averages` / `peaks` point at the LAST fired frame of channel 0 (what a reference patch reads
- * after calculate()), averagesOf(c, f) / peaksOf(c, f) at any frame of the last call. nAverages is known once both setup() and attach()
- * have happened. calculate(fftData) is kept for source compatibility: it accepts the attached transform's own magnitudes (the values are
- * already there) and rejects any other pointer -- there is no stand-alone analyser kernel. */
+/* maxiFFTOctaveAnalyzer, src/libs/maxiFFT.h:162-205, maxiFFT.cpp:201-300, used in either of two ways:
+ *  - attached to a maxiFFT (fft.attach(oct), before or after setup()): the transform's process() runs calculate() for every frame it
+ *    fires, on the device (fused into the transform at fft size 1024; at other sizes mxb_octave_process on the magnitudes it just wrote).
+ *    `averages` / `peaks` point at the LAST fired frame of channel 0 (what a reference patch reads after calculate()), averagesOf(c, f) /
+ *    peaksOf(c, f) at any frame of the last call. calculate(fftData) accepts the attached transform's own magnitudes (the values are
+ *    already there) and rejects any other pointer: process() has already run calculate() for that frame. nBandsInTheFFT must be the
+ *    transform's getNumBins(): process() refuses any other count with MXB_ERR_INVALID, at every fft size (the reference would read
+ *    past the magnitudes, or the wrong bins of every frame but the first).
+ *  - not attached: calculate(fftData) analyses the nBandsInTheFFT magnitudes it is handed, one frame per call (a host shim over
+ *    mxb_octave_process on the analyser's own context, like the per-sample maxiFFT::process), and points `averages` / `peaks` at the result.
+ * The public members keep the reference's names: peakHoldTime, peakDecayRate, linearEQIntercept and linearEQSlope are read at every
+ * process() / calculate(). nAverages is known after setup() (for an attached analyser, once its transform is set up too). The analyser
+ * owns device handles, so unlike the reference's class it cannot be copied. */
 class maxiFFTOctaveAnalyzer {
 public:
     float samplingRate = 0.f;
@@ -722,11 +728,13 @@ public:
     int peakHoldTime = 0;                                   /* setup()'s values, src/libs/maxiFFT.cpp:257-261 */
     float peakDecayRate = 0.9f, linearEQIntercept = 1.0f, linearEQSlope = 0.0f;
     maxiFFTOctaveAnalyzer() {}
-    ~maxiFFTOctaveAnalyzer() { if (h_) mxb_octave_destroy(h_); }
+    ~maxiFFTOctaveAnalyzer() { if (h_) mxb_octave_destroy(h_); if (ctx_) mxb_ctx_destroy(ctx_); }
     maxiFFTOctaveAnalyzer(const maxiFFTOctaveAnalyzer&) = delete;
-    void setup(float samplingRate_, int nBandsInTheFFT, int nAveragesPerOctave_) {
+    /* device: where an analyser that is not attached computes */
+    void setup(float samplingRate_, int nBandsInTheFFT, int nAveragesPerOctave_, int device = 0) {
         samplingRate = samplingRate_; nSpectrum = nBandsInTheFFT; nAveragesPerOctave = nAveragesPerOctave_ == 0 ? 1 : nAveragesPerOctave_;
         peakHoldTime = 0; peakDecayRate = 0.9f; linearEQIntercept = 1.0f; linearEQSlope = 0.0f;
+        device_ = device;
         isSetup_ = true;
         create();
     }
@@ -737,20 +745,34 @@ private:
     friend class maxiFFT;
     inline void create();
     maxiFFT* fft_ = nullptr;
+    mxb_ctx* ctx_ = nullptr;                                /* not attached: the analyser's own */
     mxb_octave* h_ = nullptr;
     bool isSetup_ = false;
-    int maxf_ = 0;
+    int device_ = 0, maxf_ = 0;
     std::vector<float> avg_, pk_;
 };
 
-/* maxiBarkScaleAnalyser / maxiBark, src/libs/maxiBark.h:36-128: likewise an epilogue of an attached maxiFFT (fft.attach(bark)); setup(sR, bS)
- * must name the transform's own sample rate and size. specificLoudness / relativeLoudness / totalLoudness return the values of the LAST
- * fired frame of channel 0 and accept the attached transform's magnitudes only (any other pointer is rejected); ...Of(c, f) reach the rest. */
+/* maxiBarkScaleAnalyser / maxiBark, src/libs/maxiBark.h:36-128, likewise in either of two ways:
+ *  - attached to a maxiFFT (fft.attach(bark)); setup(sR, bS) must name the transform's own sample rate and size. specificLoudness /
+ *    relativeLoudness / totalLoudness return the values of the LAST fired frame of channel 0 and accept the attached transform's
+ *    magnitudes only (any other pointer is rejected); ...Of(c, f) reach the rest.
+ *  - not attached: each of the three computes on the bS / 2 values it is handed (one frame per call, mxb_bark_process on the analyser's
+ *    own context) and returns the result.
+ * The analyser's own context and mxb_bark handle are created on first use, i.e. never for an analyser attached to a 1024-point
+ * transform (its kernel computes the loudness itself); the reference's limits (bS in 2 .. 4096, bin * sR within unsigned int) are
+ * checked then. The analyser owns device handles, so unlike the reference's class it cannot be copied. */
 template <class T>
 class maxiBarkScaleAnalyser {
 public:
     int NUM_BARK_BANDS = 24;
-    void setup(unsigned int sR, unsigned int bS) { sampleRate_ = sR; bufferSize_ = bS; isSetup_ = true; }
+    maxiBarkScaleAnalyser() {}
+    ~maxiBarkScaleAnalyser() { if (h_) mxb_bark_destroy(h_); if (ctx_) mxb_ctx_destroy(ctx_); }
+    maxiBarkScaleAnalyser(const maxiBarkScaleAnalyser&) = delete;
+    /* device: where the analyser computes when it is not fused into a 1024-point transform */
+    void setup(unsigned int sR, unsigned int bS, int device = 0) {
+        if (h_) { mxb_bark_destroy(h_); h_ = nullptr; }
+        sampleRate_ = sR; bufferSize_ = bS; device_ = device; isSetup_ = true;
+    }
     inline double* specificLoudness(const float* normalisedSpectrum);
     inline double* relativeLoudness(const float* normalisedSpectrum);
     inline double* totalLoudness(const float* normalisedSpectrum);
@@ -759,11 +781,22 @@ public:
     double totalLoudnessOf(int channel, int frame) const { return tot_[(size_t)channel * (size_t)maxf_ + (size_t)frame]; }
 private:
     friend class maxiFFT;
-    inline void own(const float* spectrum, const char* who) const;
+    inline void own(const float* spectrum, const char* who);
+    mxb_bark* handle() {
+        using maxib200_detail::check;
+        if (!h_) {
+            if (!ctx_) check(mxb_ctx_create(device_, (int32_t)maxiSettings::sampleRate, &ctx_), "mxb_ctx_create");
+            check(mxb_bark_create(ctx_, (int32_t)sampleRate_, (int32_t)bufferSize_, &h_), "mxb_bark_create");
+        }
+        return h_;
+    }
     maxiFFT* fft_ = nullptr;
+    mxb_ctx* ctx_ = nullptr;
+    mxb_bark* h_ = nullptr;
     unsigned int sampleRate_ = 0, bufferSize_ = 0;
     bool isSetup_ = false;
-    int maxf_ = 0, last_ = -1;
+    int device_ = 0, maxf_ = 0, last_ = -1;
+    std::vector<float> rows_;                               /* the fired frames of a block, packed for mxb_bark_process */
     std::vector<double> spec_, rel_, tot_;
 };
 typedef maxiBarkScaleAnalyser<double> maxiBark;
@@ -800,7 +833,8 @@ public:
         hopbuf_.clear();
         return fired;
     }
-    /* the spectral analysers of the reference as epilogues of this transform (computed by the same kernel, per fired frame) */
+    /* the spectral analysers of the reference, run by process() on every fired frame: fused into the transform's kernel at fft size
+     * 1024, on the magnitudes it wrote at other sizes */
     void attach(maxiFFTOctaveAnalyzer& o) { oct_ = &o; o.fft_ = this; if (h_) o.create(); }
     void attach(maxiBark& b) { bark_ = &b; b.fft_ = this; }
     /* magnitudes of frame f (of the last call) of channel c */
@@ -829,11 +863,14 @@ public:
         int32_t nf = 0;
         const bool post = polar && ((oct_ && oct_->h_) || bark_);
         if (!polar && (oct_ || bark_)) throw maxiError(MXB_ERR_INVALID, "maxiFFT::process: the attached analysers read magnitudes (WITH_POLAR_CONVERSION)");
+        mxb_stft_post q;
+        std::memset(&q, 0, sizeof(q));
         if (post) {
-            mxb_stft_post q;
-            std::memset(&q, 0, sizeof(q));
             if (oct_ && oct_->h_) {
                 maxiFFTOctaveAnalyzer& a = *oct_;
+                if (a.nSpectrum != bins_)
+                    throw maxiError(MXB_ERR_INVALID, "maxiFFT::process: the attached maxiFFTOctaveAnalyzer was set up for " + std::to_string(a.nSpectrum) +
+                                                     " bands; the transform has " + std::to_string(bins_) + " bins");
                 maxib200_detail::check(mxb_octave_config(a.h_, a.peakHoldTime, a.peakDecayRate, a.linearEQIntercept, a.linearEQSlope), "mxb_octave_config");
                 const size_t na = (size_t)C_ * (size_t)maxf * (size_t)(a.nAverages > 0 ? a.nAverages : 1);
                 a.avg_.resize(na); a.pk_.resize(na); a.maxf_ = maxf;
@@ -848,11 +885,21 @@ public:
                 b.spec_.resize(nb * 24); b.rel_.resize(nb * 24); b.tot_.resize(nb); b.maxf_ = maxf;
                 q.bark = 1; q.bark_specific = b.spec_.data(); q.bark_relative = b.rel_.data(); q.bark_total = b.tot_.data();
             }
+        }
+        const bool fused = post && fftSize_ == 1024;          /* the 1024-point kernel computes the analysers itself */
+        if (fused) {
             maxib200_detail::check(mxb_stft_process3(h_, values, nSamples, 1, nSamples, maxf, &o, &q, nullptr, &nf, MXB_MEM_HOST, nullptr),
                                    "mxb_stft_process3");
         } else {
             maxib200_detail::check(mxb_stft_process2(h_, values, nSamples, 1, nSamples, maxf, &o, nullptr, &nf, MXB_MEM_HOST, nullptr),
                                    "mxb_stft_process2");
+        }
+        if (post && !fused && nf > 0) {
+            /* frames 0 .. nf - 1 of every channel, in order */
+            if (q.octave)
+                maxib200_detail::check(mxb_octave_process(q.octave, mags_.data(), nf, maxf, q.octave_averages, q.octave_peaks, MXB_MEM_HOST, nullptr),
+                                       "mxb_octave_process");
+            if (q.bark) runBark(nf, maxf);
         }
         frames_ = nf; maxf_ = maxf;
         if (oct_ && oct_->h_ && nf > 0) { oct_->averages = const_cast<float*>(oct_->averagesOf(0, nf - 1)); oct_->peaks = const_cast<float*>(oct_->peaksOf(0, nf - 1)); }
@@ -875,6 +922,29 @@ public:
     int getHopSize() { return hop_; }
     int getWindowSize() { return fftSize_; }
 private:
+    /* Bark on the nf fired frames of every channel: in place when they are contiguous in the [C][maxf] layout, else packed into one
+     * call and the results put back at their rows */
+    void runBark(int nf, int maxf) {
+        maxiBark& b = *bark_;
+        const size_t n = (size_t)C_ * (size_t)nf, bins = (size_t)bins_;
+        if (C_ == 1 || nf == maxf) {
+            maxib200_detail::check(mxb_bark_process(b.handle(), mags_.data(), (int64_t)n, b.spec_.data(), b.rel_.data(), b.tot_.data(), MXB_MEM_HOST, nullptr),
+                                   "mxb_bark_process");
+            return;
+        }
+        b.rows_.resize(n * bins);
+        for (int c = 0; c < C_; ++c)
+            std::memcpy(&b.rows_[(size_t)c * nf * bins], &mags_[(size_t)c * maxf * bins], sizeof(float) * nf * bins);
+        std::vector<double> sp(n * 24), rl(n * 24), tt(n);
+        maxib200_detail::check(mxb_bark_process(b.handle(), b.rows_.data(), (int64_t)n, sp.data(), rl.data(), tt.data(), MXB_MEM_HOST, nullptr),
+                               "mxb_bark_process");
+        for (int c = 0; c < C_; ++c) {
+            const size_t src = (size_t)c * nf, dst = (size_t)c * maxf;
+            std::memcpy(&b.spec_[dst * 24], &sp[src * 24], sizeof(double) * 24 * nf);
+            std::memcpy(&b.rel_[dst * 24], &rl[src * 24], sizeof(double) * 24 * nf);
+            std::memcpy(&b.tot_[dst], &tt[src], sizeof(double) * nf);
+        }
+    }
     int C_, device_;
     mxb_ctx* ctx_ = nullptr; mxb_stft* h_ = nullptr;
     int fftSize_ = 0, hop_ = 0, bins_ = 0, frames_ = 0, maxf_ = 0;
@@ -884,18 +954,38 @@ private:
 };
 
 inline void maxiFFTOctaveAnalyzer::create() {
-    if (!isSetup_ || !fft_ || !fft_->context()) return;
+    using maxib200_detail::check;
+    if (!isSetup_ || (fft_ && !fft_->context())) return;
     if (h_) { mxb_octave_destroy(h_); h_ = nullptr; }
-    maxib200_detail::check(mxb_octave_create(fft_->context(), fft_->channels(), samplingRate, nSpectrum, nAveragesPerOctave, &h_), "mxb_octave_create");
+    if (!fft_ && !ctx_) check(mxb_ctx_create(device_, (int32_t)maxiSettings::sampleRate, &ctx_), "mxb_ctx_create");
+    check(mxb_octave_create(fft_ ? fft_->context() : ctx_, fft_ ? fft_->channels() : 1, samplingRate, nSpectrum, nAveragesPerOctave, &h_), "mxb_octave_create");
     nAverages = mxb_octave_n_averages(h_);
+    if (!fft_) {      /* the results of calculate(): one frame of one channel */
+        avg_.assign((size_t)nAverages, 0.f); pk_.assign((size_t)nAverages, 0.f); maxf_ = 1;
+        averages = avg_.data(); peaks = pk_.data();
+    }
 }
 inline void maxiFFTOctaveAnalyzer::calculate(const float* fftData) {
-    if (!h_ || !fft_ || fft_->frames() <= 0) throw maxiError(MXB_ERR_STATE, "maxiFFTOctaveAnalyzer::calculate: attach the analyser to a maxiFFT; its process() runs it per frame");
+    using maxib200_detail::check;
+    if (!fft_) {
+        if (!h_) throw maxiError(MXB_ERR_STATE, "maxiFFTOctaveAnalyzer::calculate before setup()");
+        check(mxb_octave_config(h_, peakHoldTime, peakDecayRate, linearEQIntercept, linearEQSlope), "mxb_octave_config");
+        check(mxb_octave_process(h_, fftData, 1, 1, avg_.data(), pk_.data(), MXB_MEM_HOST, nullptr), "mxb_octave_process");
+        averages = avg_.data(); peaks = pk_.data();
+        return;
+    }
+    if (!h_ || fft_->frames() <= 0) throw maxiError(MXB_ERR_STATE, "maxiFFTOctaveAnalyzer::calculate: the attached maxiFFT has fired no frame; its process() runs the analyser per frame");
     if (fftData != fft_->magnitudesOf(0, fft_->frames() - 1) && fftData != fft_->magnitudesOf(0, 0))
-        throw maxiError(MXB_ERR_UNSUPPORTED, "maxiFFTOctaveAnalyzer::calculate: only the attached transform's own magnitudes can be analysed");
+        throw maxiError(MXB_ERR_UNSUPPORTED, "maxiFFTOctaveAnalyzer::calculate: an attached analyser has analysed its transform's frame already; only those magnitudes can be passed");
 }
-template <class T> inline void maxiBarkScaleAnalyser<T>::own(const float* spectrum, const char* who) const {
-    if (!fft_ || last_ < 0) throw maxiError(MXB_ERR_STATE, std::string(who) + ": attach the analyser to a maxiFFT; its process() runs it per frame");
+template <class T> inline void maxiBarkScaleAnalyser<T>::own(const float* spectrum, const char* who) {
+    if (!fft_) {      /* not attached: analyse the spectrum handed in */
+        if (!isSetup_) throw maxiError(MXB_ERR_STATE, std::string(who) + " before setup()");
+        spec_.resize(24); rel_.resize(24); tot_.resize(1); maxf_ = 1; last_ = 0;
+        maxib200_detail::check(mxb_bark_process(handle(), spectrum, 1, spec_.data(), rel_.data(), tot_.data(), MXB_MEM_HOST, nullptr), "mxb_bark_process");
+        return;
+    }
+    if (last_ < 0) throw maxiError(MXB_ERR_STATE, std::string(who) + ": the attached maxiFFT has fired no frame; its process() runs the analyser per frame");
     if (spectrum != fft_->magnitudesOf(0, last_) && spectrum != fft_->magnitudesOf(0, 0))
         throw maxiError(MXB_ERR_UNSUPPORTED, std::string(who) + ": only the attached transform's own magnitudes can be analysed");
 }

@@ -34,6 +34,7 @@ EXPORTS = [
     "mxb_ctx_set_tables", "mxb_patch_create", "mxb_patch_destroy", "mxb_patch_set_param", "mxb_patch_set_state", "mxb_patch_get_state",
     "mxb_patch_get_ring", "mxb_patch_process", "mxb_patch_launch_count", "mxb_patch_set_mode", "mxb_patch_get_mode", "mxb_patch_codegen",
     "mxb_patch_create2",
+    "mxb_octave_process", "mxb_bark_create", "mxb_bark_destroy", "mxb_bark_process",
 ]
 
 
@@ -135,6 +136,10 @@ def lib():
         "mxb_patch_get_mode": (i32, [vp]),
         "mxb_patch_codegen": (i32, [vp, vp, i64, vp, i32]),
         "mxb_patch_create2": (i32, [vp, vp, i32, vp, pp]),
+        "mxb_octave_process": (i32, [vp, vp, i32, i32, vp, vp, i32, vp]),
+        "mxb_bark_create": (i32, [vp, i32, i32, pp]),
+        "mxb_bark_destroy": (i32, [vp]),
+        "mxb_bark_process": (i32, [vp, vp, i64, vp, vp, vp, i32, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = the library does not export a declared symbol
@@ -464,16 +469,33 @@ class StftPost(C.Structure):
 
 
 class Octave:
-    """mxb_octave: maxiFFTOctaveAnalyzer::setup for every channel of one Stft (state: averages, peaks, hold times on the device)."""
+    """mxb_octave: maxiFFTOctaveAnalyzer::setup for every channel of one Stft (state: averages, peaks, hold times on the device). The
+    state is shared by the transform's fused epilogue (stft_process_post) and process() on spectra in memory."""
 
     def __init__(self, channels, sampling_rate, n_bands, n_per_octave, ctx=None, device=0, sample_rate=48000):
         self.ctx = ctx or default_context(device, sample_rate)
         self.h = C.c_void_p()
         check(lib().mxb_octave_create(self.ctx.h, int(channels), float(sampling_rate), int(n_bands), int(n_per_octave), C.byref(self.h)), "mxb_octave_create")
-        self.C, self.n_averages = int(channels), int(lib().mxb_octave_n_averages(self.h))
+        self.C, self.bands, self.n_averages = int(channels), int(n_bands), int(lib().mxb_octave_n_averages(self.h))
 
     def config(self, peak_hold_time=0, peak_decay_rate=0.9, eq_intercept=1.0, eq_slope=0.0):
         check(lib().mxb_octave_config(self.h, int(peak_hold_time), float(peak_decay_rate), float(eq_intercept), float(eq_slope)), "mxb_octave_config")
+
+    def process(self, mags):
+        """maxiFFTOctaveAnalyzer::calculate on every frame of float32 [C][frames][n_bands] host magnitudes, frames in order ->
+        (averages, peaks) float32 [C][frames][nAverages] (mxb_octave_process)."""
+        m = np.ascontiguousarray(mags, dtype=np.float32)
+        if m.ndim != 3 or m.shape[0] != self.C or m.shape[2] != self.bands:
+            raise MxbError(f"Octave.process: magnitudes of shape {m.shape}, expected ({self.C}, frames, {self.bands})")
+        f = m.shape[1]
+        av = np.zeros((self.C, f, self.n_averages), dtype=np.float32); pk = np.zeros_like(av)
+        check(lib().mxb_octave_process(self.h, _np_ptr(m), f, f, _np_ptr(av), _np_ptr(pk), MEM_HOST, None), "mxb_octave_process")
+        return av, pk
+
+    def process_device(self, mags_ptr, frames, max_frames, averages_ptr=None, peaks_ptr=None, stream=0):
+        """Device pointers (layout of mxb_octave_process), asynchronous on `stream` (a raw cudaStream_t value)."""
+        check(lib().mxb_octave_process(self.h, _ptr(mags_ptr), int(frames), int(max_frames), _ptr(averages_ptr), _ptr(peaks_ptr), MEM_DEVICE,
+                                       C.c_void_p(int(stream)) if stream else None), "mxb_octave_process")
 
     def close(self):
         if getattr(self, "h", None):
@@ -509,6 +531,44 @@ def stft_process_post(st, x, octave=None, bark=False):
     if bark:
         r.update(bark_specific=bs[:, :f].copy(), bark_relative=br[:, :f].copy(), bark_total=bt[:, :f].copy())
     return r
+
+
+class Bark:
+    """mxb_bark: maxiBarkScaleAnalyser::setup(sample_rate, buffer_size) + specificLoudness / relativeLoudness / totalLoudness on any
+    spectrum of buffer_size / 2 bins."""
+
+    def __init__(self, sample_rate, buffer_size, ctx=None, device=0):
+        self.ctx = ctx or default_context(device)           # the band limits come from sample_rate, not from the context's rate
+        self.sample_rate, self.buffer_size, self.bins = int(sample_rate), int(buffer_size), int(buffer_size) // 2
+        self.h = C.c_void_p()
+        check(lib().mxb_bark_create(self.ctx.h, self.sample_rate, self.buffer_size, C.byref(self.h)), "mxb_bark_create")
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().mxb_bark_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def process(self, spectrum):
+        """float32 [..., buffer_size / 2] host array -> (specific [..., 24], relative [..., 24], total [...]) float64."""
+        m = np.ascontiguousarray(spectrum, dtype=np.float32)
+        if m.ndim < 1 or m.shape[-1] != self.bins:
+            raise MxbError(f"Bark.process: spectra of shape {m.shape}, expected (..., {self.bins})")
+        lead = m.shape[:-1]
+        n = int(np.prod(lead)) if lead else 1
+        sp = np.empty((n, 24)); rl = np.empty((n, 24)); tt = np.empty(n)
+        check(lib().mxb_bark_process(self.h, _np_ptr(m), n, _np_ptr(sp), _np_ptr(rl), _np_ptr(tt), MEM_HOST, None), "mxb_bark_process")
+        return sp.reshape(lead + (24,)), rl.reshape(lead + (24,)), tt.reshape(lead)
+
+    def process_device(self, spectrum_ptr, n, specific_ptr=None, relative_ptr=None, total_ptr=None, stream=0):
+        """Device pointers (layout of mxb_bark_process), asynchronous on `stream` (a raw cudaStream_t value)."""
+        check(lib().mxb_bark_process(self.h, _ptr(spectrum_ptr), int(n), _ptr(specific_ptr), _ptr(relative_ptr), _ptr(total_ptr), MEM_DEVICE,
+                                     C.c_void_p(int(stream)) if stream else None), "mxb_bark_process")
 
 
 class Mfcc:
