@@ -485,20 +485,26 @@ private:
     maxiArg cutoff_{1000.0}, res_{1.0};        /* maxiSVF ctor: setParams(1000, 1), src/maximilian.h:1284 */
 };
 
-/* maxiBiquad, src/maximilian.h:1343-1486 */
+/* maxiBiquad, src/maximilian.h:1343-1486. The reference's constructor designs nothing: until set() runs, every coefficient is 0
+ * (:1482) and play() returns 0 while its state follows the input. No stage computes that, so play() before set() throws
+ * maxiError(MXB_ERR_UNSUPPORTED) instead of inventing a design. */
 class maxiBiquad {
 public:
     enum filterTypes { LOWPASS, HIGHPASS, BANDPASS, NOTCH, PEAK, LOWSHELF, HIGHSHELF };
     explicit maxiBiquad(maxiVoices& v) : v_(&v) {}
-    void set(filterTypes filtType, const maxiArg& cutoff, const maxiArg& Q, const maxiArg& peakGain) { type_ = (int)filtType; cutoff_ = cutoff; q_ = Q; gain_ = peakGain; }
+    void set(filterTypes filtType, const maxiArg& cutoff, const maxiArg& Q, const maxiArg& peakGain) {
+        type_ = (int)filtType; cutoff_ = cutoff; q_ = Q; gain_ = peakGain; set_ = true;
+    }
     maxiSignal play(maxiSignal input) {
         v_->check(input, "maxiBiquad::play");
+        if (!set_) throw maxiError(MXB_ERR_UNSUPPORTED, "maxiBiquad::play: set() was never called (the reference's coefficients are all 0)");
         return v_->emit(MXB_OP_BIQUAD, type_, {input.src, cutoff_.op(v_), q_.op(v_), gain_.op(v_)}, true, 3);
     }
 private:
     maxiVoices* v_;
     int type_ = 0;
-    maxiArg cutoff_{1000.0}, q_{1.0}, gain_{0.0};
+    bool set_ = false;
+    maxiArg cutoff_{0.0}, q_{0.0}, gain_{0.0};
 };
 
 /* maxiEnv (ADSR / AR), src/maximilian.h:888-932 / src/maximilian.cpp:1319-1494. The trigger is an argument here (the reference's
