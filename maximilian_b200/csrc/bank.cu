@@ -22,30 +22,38 @@ struct mxb_bank {
     double* dp[MXB_P_COUNT];                 // device copies: the buffer the next block reads (== dp_buf[id][dp_cur[id]])
     // Block-rate control data uploaded with mxb_bank_set_param_async from host memory is double-buffered: the copy of block
     // k+1's values runs on a private copy stream into the buffer block k is NOT reading, so it overlaps block k's kernel.
-    double* dp_buf[MXB_P_COUNT][2];          // [1] allocated on first asynchronous host upload
+    DevBuf<double> dp_buf[MXB_P_COUNT][2];   // [1] allocated on first asynchronous host upload
     int dp_cur[MXB_P_COUNT];
     bool dp_pending[MXB_P_COUNT];            // an upload into dp_buf[id][1 - cur] is in flight: the next block flips to it
     cudaEvent_t ev_up[MXB_P_COUNT];          // upload finished (copy stream)
     cudaEvent_t ev_read[MXB_P_COUNT][2];     // last kernel that read dp_buf[id][k] finished (process stream)
     bool ev_read_set[MXB_P_COUNT][2];
     cudaStream_t up_stream;
-    double* osc_out;
-    double *f0, *f1, *f2, *cf[5];
-    double *env_amp, *env_output;
-    long long *env_holdcount, *env_hold;
-    int* env_flags;
-    int *trig_on, *trig_off;                 // staging for MXB_MEM_HOST gates
-    int *dl_phase, *dl_size, *dl_pos;
-    double* ring;                            // [V][delay_taps]
-    double* partials; size_t partials_len;
-    double* mix_dev;                         // [max_frames][2]
-    unsigned char* out_stage; size_t out_stage_len;   // staging for MXB_MEM_HOST out (bytes: fp64 or fp32)
-    double* fm_stage; size_t fm_stage_len;   // staging for host-resident per-sample frequencies
-    double* cm_stage; size_t cm_stage_len;   // ... and cutoffs
-    double* ds_stage; size_t ds_stage_len;   // ... and delay sizes
-    unsigned char* tv_stage; size_t tv_stage_len;     // ... and per-sample triggers
+    DevBuf<double> osc_out;
+    DevBuf<double> f0, f1, f2, cf[5];
+    DevBuf<double> env_amp, env_output;
+    DevBuf<long long> env_holdcount, env_hold;
+    DevBuf<int> env_flags;
+    DevBuf<int> trig_on, trig_off;           // staging for MXB_MEM_HOST gates
+    DevBuf<int> dl_phase, dl_size, dl_pos;
+    DevBuf<double> ring;                     // [V][delay_taps]
+    DevBuf<double> partials;
+    DevBuf<double> mix_dev;                  // [max_frames][2]
+    DevBuf<unsigned char> out_stage;         // staging for MXB_MEM_HOST out (bytes: fp64 or fp32)
+    DevBuf<double> fm_stage;                 // staging for host-resident per-sample frequencies
+    DevBuf<double> cm_stage;                 // ... and cutoffs
+    DevBuf<double> ds_stage;                 // ... and delay sizes
+    DevBuf<unsigned char> tv_stage;          // ... and per-sample triggers
     int64_t launches;
     mxb_exchange* ex;                        // peer-memory mix exchange (multi-GPU), or NULL
+
+    ~mxb_bank() {
+        for (int i = 0; i < MXB_P_COUNT; ++i) {
+            if (ev_up[i]) cudaEventDestroy(ev_up[i]);
+            for (auto e : ev_read[i]) if (e) cudaEventDestroy(e);
+        }
+        if (up_stream) cudaStreamDestroy(up_stream);
+    }
 };
 
 namespace {
@@ -95,7 +103,7 @@ int redesign(mxb_bank* b) {
         for (int i = 0; i < nt; ++i) ts.emplace_back(part, (int)((long long)b->V * i / nt), (int)((long long)b->V * (i + 1) / nt));
         for (auto& t : ts) t.join();
     }
-    for (int i = 0; i < 5; ++i) MXB_CUDA(cudaMemcpy(b->cf[i], cf[i].data(), sizeof(double) * (size_t)b->V, cudaMemcpyHostToDevice));
+    for (int i = 0; i < 5; ++i) MXB_CUDA(cudaMemcpy(b->cf[i].get(), cf[i].data(), sizeof(double) * (size_t)b->V, cudaMemcpyHostToDevice));
     return MXB_OK;
 }
 
@@ -106,21 +114,17 @@ __global__ void ring_linear_kernel(double* __restrict__ ring, size_t V, size_t v
     if (set) ring[dl_slot(V, voice, r)] = lin[r]; else lin[r] = ring[dl_slot(V, voice, r)];
 }
 
-int free_bank(mxb_bank* b) {
-    if (!b) return MXB_OK;
-    for (int i = 0; i < MXB_P_COUNT; ++i) {
-        cudaFree(b->dp_buf[i][0]); cudaFree(b->dp_buf[i][1]);
-        if (b->ev_up[i]) cudaEventDestroy(b->ev_up[i]);
-        for (int k = 0; k < 2; ++k) if (b->ev_read[i][k]) cudaEventDestroy(b->ev_read[i][k]);
+// the fp64 state array of a state id (MXB_S_*), or NULL for the integer ones and unknown ids
+double* f64_state(mxb_bank* b, int32_t id) {
+    switch (id) {
+        case MXB_S_FILT_0: return b->f0.get();
+        case MXB_S_FILT_1: return b->f1.get();
+        case MXB_S_FILT_2: return b->f2.get();
+        case MXB_S_ENV_AMPLITUDE: return b->env_amp.get();
+        case MXB_S_ENV_OUTPUT: return b->env_output.get();
+        case MXB_S_OSC_OUTPUT: return b->osc_out.get();
+        default: return nullptr;
     }
-    if (b->up_stream) cudaStreamDestroy(b->up_stream);
-    cudaFree(b->osc_out); cudaFree(b->f0); cudaFree(b->f1); cudaFree(b->f2);
-    for (int i = 0; i < 5; ++i) cudaFree(b->cf[i]);
-    cudaFree(b->env_amp); cudaFree(b->env_output); cudaFree(b->env_holdcount); cudaFree(b->env_hold); cudaFree(b->env_flags);
-    cudaFree(b->trig_on); cudaFree(b->trig_off); cudaFree(b->dl_phase); cudaFree(b->dl_size); cudaFree(b->dl_pos); cudaFree(b->ring);
-    cudaFree(b->partials); cudaFree(b->mix_dev); cudaFree(b->out_stage); cudaFree(b->fm_stage); cudaFree(b->cm_stage); cudaFree(b->ds_stage); cudaFree(b->tv_stage);
-    delete b;
-    return MXB_OK;
 }
 
 int upload_fill(double* dst, size_t n, double value) {
@@ -146,47 +150,44 @@ int32_t mxb_bank_create(mxb_ctx* ctx, const mxb_bank_desc* d, mxb_bank** out) {
     MXB_REQUIRE(d->max_frames > 0, MXB_ERR_INVALID, "mxb_bank_create: max_frames %d", d->max_frames);
     DeviceGuard g(ctx->device);
     MXB_REQUIRE(g.ok, MXB_ERR_CUDA, "mxb_bank_create: cudaSetDevice failed");
-    mxb_bank* b = new (std::nothrow) mxb_bank();
+    std::unique_ptr<mxb_bank> b(new (std::nothrow) mxb_bank());
     MXB_REQUIRE(b, MXB_ERR_ALLOC, "mxb_bank_create: out of host memory");
     b->ctx = ctx; b->desc = *d; b->V = d->voices;           // every other member is value-initialised: zero / NULL
     const size_t V = (size_t)d->voices;
     int rc = MXB_OK;
-#define TRY(x) do { rc = (x); if (rc != MXB_OK) { free_bank(b); return rc; } } while (0)
     static const double defaults[MXB_P_COUNT] = {0, 0, 0.5, 1000.0, 1.0, 0, 0, 0, 0, 0, 1.0, 1.0, 0, 0.5, 0, 0, 1.0};
-    for (int i = 0; i < MXB_P_COUNT; ++i) {
-        TRY(dev_alloc(&b->dp_buf[i][0], V));
-        b->dp[i] = b->dp_buf[i][0];
+    for (int i = 0; i < MXB_P_COUNT && rc == MXB_OK; ++i) {
+        rc = b->dp_buf[i][0].alloc(V);
+        b->dp[i] = b->dp_buf[i][0].get();
         b->hp[i].assign(V, defaults[i]);
-        if (defaults[i] != 0.0) TRY(upload_fill(b->dp[i], V, defaults[i]));
+        if (rc == MXB_OK && defaults[i] != 0.0) rc = upload_fill(b->dp[i], V, defaults[i]);
     }
-    TRY(dev_alloc(&b->osc_out, V));
-    TRY(dev_alloc(&b->f0, V)); TRY(dev_alloc(&b->f1, V)); TRY(dev_alloc(&b->f2, V));
-    for (int i = 0; i < 5; ++i) TRY(dev_alloc(&b->cf[i], V));
-    TRY(dev_alloc(&b->env_amp, V)); TRY(dev_alloc(&b->env_output, V));
-    TRY(dev_alloc(&b->env_holdcount, V)); TRY(dev_alloc(&b->env_hold, V)); TRY(dev_alloc(&b->env_flags, V));
-    {
-        std::vector<long long> one(V, 1);   // maxiEnv::holdtime = 1, src/maximilian.h:913
-        cudaError_t e = cudaMemcpy(b->env_hold, one.data(), sizeof(long long) * V, cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) { set_error("cudaMemcpy: %s", cudaGetErrorString(e)); free_bank(b); return MXB_ERR_CUDA; }
+    if (rc == MXB_OK) rc = b->osc_out.alloc(V);
+    if (rc == MXB_OK) rc = b->f0.alloc(V);
+    if (rc == MXB_OK) rc = b->f1.alloc(V);
+    if (rc == MXB_OK) rc = b->f2.alloc(V);
+    for (int i = 0; i < 5 && rc == MXB_OK; ++i) rc = b->cf[i].alloc(V);
+    if (rc == MXB_OK) rc = b->env_amp.alloc(V);
+    if (rc == MXB_OK) rc = b->env_output.alloc(V);
+    if (rc == MXB_OK) rc = b->env_holdcount.alloc(V);
+    if (rc == MXB_OK) rc = b->env_flags.alloc(V);
+    if (rc == MXB_OK) rc = b->env_hold.upload(std::vector<long long>(V, 1));      // maxiEnv::holdtime = 1, src/maximilian.h:913
+    if (rc == MXB_OK) rc = b->trig_on.alloc(V);
+    if (rc == MXB_OK) rc = b->trig_off.alloc(V);
+    if (rc == MXB_OK) rc = b->mix_dev.alloc((size_t)d->max_frames * 2);
+    if (rc == MXB_OK && d->delay_taps > 0) {
+        rc = b->dl_phase.alloc(V);
+        if (rc == MXB_OK) rc = b->dl_pos.alloc(V);
+        if (rc == MXB_OK) rc = b->dl_size.upload(std::vector<int>(V, 1));
+        if (rc == MXB_OK) rc = b->ring.alloc(dl_ring_doubles(V, d->delay_taps));   // zeroed: maxiDelayline ctor memset, src/maximilian.cpp:415-417
     }
-    TRY(dev_alloc(&b->trig_on, V)); TRY(dev_alloc(&b->trig_off, V));
-    TRY(dev_alloc(&b->mix_dev, (size_t)d->max_frames * 2));
-    if (d->delay_taps > 0) {
-        TRY(dev_alloc(&b->dl_phase, V));
-        TRY(dev_alloc(&b->dl_size, V));
-        TRY(dev_alloc(&b->dl_pos, V));
-        std::vector<int> one(V, 1);
-        cudaError_t e = cudaMemcpy(b->dl_size, one.data(), sizeof(int) * V, cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) { set_error("cudaMemcpy: %s", cudaGetErrorString(e)); free_bank(b); return MXB_ERR_CUDA; }
-        TRY(dev_alloc(&b->ring, dl_ring_doubles(V, d->delay_taps)));   // zeroed: maxiDelayline ctor memset, src/maximilian.cpp:415-417
-    }
-    if (d->filt_kind == MXB_FILT_SVF) {          // maxiSVF ctor: setParams(1000, 1), src/maximilian.h:1284
+    if (rc == MXB_OK && d->filt_kind == MXB_FILT_SVF) {          // maxiSVF ctor: setParams(1000, 1), src/maximilian.h:1284
         b->set_mask[MXB_P_CUTOFF] = b->set_mask[MXB_P_RESONANCE] = true;
-        TRY(redesign(b));
+        rc = redesign(b.get());
         b->set_mask[MXB_P_CUTOFF] = b->set_mask[MXB_P_RESONANCE] = false;
     }
-#undef TRY
-    *out = b;
+    if (rc != MXB_OK) return rc;
+    *out = b.release();
     return MXB_OK;
 }
 
@@ -194,7 +195,8 @@ int32_t mxb_bank_destroy(mxb_bank* b) {
     if (!b) return MXB_OK;
     DeviceGuard g(b->ctx->device);
     cudaDeviceSynchronize();
-    return free_bank(b);
+    delete b;
+    return MXB_OK;
 }
 
 int32_t mxb_bank_voices(const mxb_bank* b) { return b ? b->V : MXB_ERR_INVALID; }
@@ -236,16 +238,16 @@ int32_t mxb_bank_set_param(mxb_bank* b, int32_t id, const double* values, int32_
             MXB_REQUIRE(fabs(b->hp[id][v]) < 2147483648.0, MXB_ERR_INVALID, "mxb_bank_set_param: holdtime %.0f of voice %zu does not fit 32 bits", b->hp[id][v], v);
             h[v] = (long long)b->hp[id][v];
         }
-        MXB_CUDA(cudaMemcpy(b->env_hold, h.data(), sizeof(long long) * V, cudaMemcpyHostToDevice));
-    } else if (id == MXB_P_DELAY_POSITION && b->dl_pos) {
+        MXB_CUDA(cudaMemcpy(b->env_hold.get(), h.data(), sizeof(long long) * V, cudaMemcpyHostToDevice));
+    } else if (id == MXB_P_DELAY_POSITION && b->dl_pos.get()) {
         std::vector<int> h(V);
         for (size_t v = 0; v < V; ++v) {
             const double s = b->hp[id][v];
             MXB_REQUIRE(fabs(s) < 2147483648.0, MXB_ERR_INVALID, "mxb_bank_set_param: delay position %.0f of voice %zu does not fit an int", s, v);
             h[v] = (int)s;
         }
-        MXB_CUDA(cudaMemcpy(b->dl_pos, h.data(), sizeof(int) * V, cudaMemcpyHostToDevice));
-    } else if (id == MXB_P_DELAY_SIZE && b->dl_size) {
+        MXB_CUDA(cudaMemcpy(b->dl_pos.get(), h.data(), sizeof(int) * V, cudaMemcpyHostToDevice));
+    } else if (id == MXB_P_DELAY_SIZE && b->dl_size.get()) {
         std::vector<int> h(V);
         for (size_t v = 0; v < V; ++v) {
             const double s = b->hp[id][v];
@@ -254,7 +256,7 @@ int32_t mxb_bank_set_param(mxb_bank* b, int32_t id, const double* values, int32_
                         "mxb_bank_set_param: delay size %g of voice %zu is not an int <= delay_taps %d", s, v, b->desc.delay_taps);
             h[v] = (int)s;
         }
-        MXB_CUDA(cudaMemcpy(b->dl_size, h.data(), sizeof(int) * V, cudaMemcpyHostToDevice));
+        MXB_CUDA(cudaMemcpy(b->dl_size.get(), h.data(), sizeof(int) * V, cudaMemcpyHostToDevice));
     }
     return MXB_OK;
 }
@@ -283,9 +285,9 @@ int32_t mxb_bank_set_param_async(mxb_bank* b, int32_t id, const double* values, 
     if (!b->up_stream) MXB_CUDA(cudaStreamCreateWithFlags(&b->up_stream, cudaStreamNonBlocking));
     if (!b->ev_up[id]) MXB_CUDA(cudaEventCreateWithFlags(&b->ev_up[id], cudaEventDisableTiming));
     const int tgt = 1 - b->dp_cur[id];
-    if (!b->dp_buf[id][tgt]) { int rc = dev_alloc(&b->dp_buf[id][tgt], (size_t)b->V, false); if (rc != MXB_OK) return rc; }
+    if (!b->dp_buf[id][tgt].get()) { int rc = b->dp_buf[id][tgt].alloc((size_t)b->V, false); if (rc != MXB_OK) return rc; }
     if (b->ev_read_set[id][tgt]) MXB_CUDA(cudaStreamWaitEvent(b->up_stream, b->ev_read[id][tgt], 0));
-    MXB_CUDA(cudaMemcpyAsync(b->dp_buf[id][tgt], values, bytes, cudaMemcpyHostToDevice, b->up_stream));
+    MXB_CUDA(cudaMemcpyAsync(b->dp_buf[id][tgt].get(), values, bytes, cudaMemcpyHostToDevice, b->up_stream));
     MXB_CUDA(cudaEventRecord(b->ev_up[id], b->up_stream));
     b->dp_pending[id] = true;
     b->set_mask[id] = true;
@@ -299,23 +301,16 @@ int32_t mxb_bank_get_state(mxb_bank* b, int32_t id, double* values, int32_t mem)
     MXB_CUDA(cudaDeviceSynchronize());
     const size_t V = (size_t)b->V;
     const cudaMemcpyKind kind = mem == MXB_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
-    const double* src = nullptr;
-    if (id >= 0 && id < MXB_P_COUNT) src = b->dp[id];
-    else if (id == MXB_S_FILT_0) src = b->f0;
-    else if (id == MXB_S_FILT_1) src = b->f1;
-    else if (id == MXB_S_FILT_2) src = b->f2;
-    else if (id == MXB_S_ENV_AMPLITUDE) src = b->env_amp;
-    else if (id == MXB_S_ENV_OUTPUT) src = b->env_output;
-    else if (id == MXB_S_OSC_OUTPUT) src = b->osc_out;
+    const double* src = id >= 0 && id < MXB_P_COUNT ? b->dp[id] : f64_state(b, id);
     if (src) { MXB_CUDA(cudaMemcpy(values, src, sizeof(double) * V, kind)); return MXB_OK; }
     // integer state, returned as doubles
     std::vector<double> h(V, 0.0);
     if (id == MXB_S_ENV_HOLDCOUNT) {
         std::vector<long long> t(V);
-        MXB_CUDA(cudaMemcpy(t.data(), b->env_holdcount, sizeof(long long) * V, cudaMemcpyDeviceToHost));
+        MXB_CUDA(cudaMemcpy(t.data(), b->env_holdcount.get(), sizeof(long long) * V, cudaMemcpyDeviceToHost));
         for (size_t v = 0; v < V; ++v) h[v] = (double)t[v];
     } else if (id == MXB_S_ENV_FLAGS || id == MXB_S_DELAY_PHASE) {
-        const int* s = id == MXB_S_ENV_FLAGS ? b->env_flags : b->dl_phase;
+        const int* s = id == MXB_S_ENV_FLAGS ? b->env_flags.get() : b->dl_phase.get();
         if (s) {
             std::vector<int> t(V);
             MXB_CUDA(cudaMemcpy(t.data(), s, sizeof(int) * V, cudaMemcpyDeviceToHost));
@@ -331,40 +326,41 @@ int32_t mxb_bank_get_state(mxb_bank* b, int32_t id, double* values, int32_t mem)
 
 int32_t mxb_bank_get_ring(mxb_bank* b, int32_t voice, double* dst, int32_t n, int32_t mem) {
     MXB_REQUIRE(b && dst, MXB_ERR_INVALID, "mxb_bank_get_ring: NULL argument");
-    MXB_REQUIRE(b->ring, MXB_ERR_STATE, "mxb_bank_get_ring: bank has no delay line");
+    MXB_REQUIRE(b->ring.get(), MXB_ERR_STATE, "mxb_bank_get_ring: bank has no delay line");
     MXB_REQUIRE(voice >= 0 && voice < b->V && n >= 0 && n <= b->desc.delay_taps, MXB_ERR_INVALID, "mxb_bank_get_ring: voice %d n %d", voice, n);
     MXB_REQUIRE(mem == MXB_MEM_HOST || mem == MXB_MEM_DEVICE, MXB_ERR_INVALID, "mxb_bank_get_ring: mem %d", mem);
     if (n == 0) return MXB_OK;
     DeviceGuard g(b->ctx->device);
     // the ring is chunk-interleaved and swizzled (delay_kernels.cuh): one small kernel walks the voice's slots
+    DevBuf<double> tmp;
     double* d_lin = dst;
-    if (mem == MXB_MEM_HOST) { int rc = dev_alloc(&d_lin, (size_t)n, false); if (rc != MXB_OK) return rc; }
-    ring_linear_kernel<<<(n + 255) / 256, 256>>>(b->ring, (size_t)b->V, (size_t)voice, d_lin, n, 0);
+    if (mem == MXB_MEM_HOST) { int rc = tmp.alloc((size_t)n, false); if (rc != MXB_OK) return rc; d_lin = tmp.get(); }
+    ring_linear_kernel<<<(n + 255) / 256, 256>>>(b->ring.get(), (size_t)b->V, (size_t)voice, d_lin, n, 0);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess && mem == MXB_MEM_HOST) e = cudaMemcpy(dst, d_lin, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost);
     else if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (mem == MXB_MEM_HOST) cudaFree(d_lin);
     if (e != cudaSuccess) { set_error("mxb_bank_get_ring: %s", cudaGetErrorString(e)); return MXB_ERR_CUDA; }
     return MXB_OK;
 }
 
 int32_t mxb_bank_set_ring(mxb_bank* b, int32_t voice, const double* src, int32_t n, int32_t mem) {
     MXB_REQUIRE(b && src, MXB_ERR_INVALID, "mxb_bank_set_ring: NULL argument");
-    MXB_REQUIRE(b->ring, MXB_ERR_STATE, "mxb_bank_set_ring: bank has no delay line");
+    MXB_REQUIRE(b->ring.get(), MXB_ERR_STATE, "mxb_bank_set_ring: bank has no delay line");
     MXB_REQUIRE(voice >= 0 && voice < b->V && n >= 0 && n <= b->desc.delay_taps, MXB_ERR_INVALID, "mxb_bank_set_ring: voice %d n %d", voice, n);
     MXB_REQUIRE(mem == MXB_MEM_HOST || mem == MXB_MEM_DEVICE, MXB_ERR_INVALID, "mxb_bank_set_ring: mem %d", mem);
     if (n == 0) return MXB_OK;
     DeviceGuard g(b->ctx->device);
+    DevBuf<double> tmp;
     double* d_lin = const_cast<double*>(src);
     if (mem == MXB_MEM_HOST) {
-        int rc = dev_alloc(&d_lin, (size_t)n, false); if (rc != MXB_OK) return rc;
+        int rc = tmp.alloc((size_t)n, false); if (rc != MXB_OK) return rc;
+        d_lin = tmp.get();
         cudaError_t e0 = cudaMemcpy(d_lin, src, sizeof(double) * (size_t)n, cudaMemcpyHostToDevice);
-        if (e0 != cudaSuccess) { cudaFree(d_lin); set_error("mxb_bank_set_ring: %s", cudaGetErrorString(e0)); return MXB_ERR_CUDA; }
+        if (e0 != cudaSuccess) { set_error("mxb_bank_set_ring: %s", cudaGetErrorString(e0)); return MXB_ERR_CUDA; }
     }
-    ring_linear_kernel<<<(n + 255) / 256, 256>>>(b->ring, (size_t)b->V, (size_t)voice, d_lin, n, 1);
+    ring_linear_kernel<<<(n + 255) / 256, 256>>>(b->ring.get(), (size_t)b->V, (size_t)voice, d_lin, n, 1);
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
-    if (mem == MXB_MEM_HOST) cudaFree(d_lin);
     if (e != cudaSuccess) { set_error("mxb_bank_set_ring: %s", cudaGetErrorString(e)); return MXB_ERR_CUDA; }
     return MXB_OK;
 }
@@ -375,13 +371,7 @@ int32_t mxb_bank_set_state(mxb_bank* b, int32_t id, const double* values, int32_
     DeviceGuard g(b->ctx->device);
     MXB_CUDA(cudaDeviceSynchronize());
     const size_t V = (size_t)b->V;
-    double* dst = nullptr;
-    if (id == MXB_S_FILT_0) dst = b->f0;
-    else if (id == MXB_S_FILT_1) dst = b->f1;
-    else if (id == MXB_S_FILT_2) dst = b->f2;
-    else if (id == MXB_S_ENV_AMPLITUDE) dst = b->env_amp;
-    else if (id == MXB_S_ENV_OUTPUT) dst = b->env_output;
-    else if (id == MXB_S_OSC_OUTPUT) dst = b->osc_out;
+    double* dst = f64_state(b, id);
     if (dst) {
         MXB_CUDA(cudaMemcpy(dst, values, sizeof(double) * V, mem == MXB_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice));
         return MXB_OK;
@@ -396,9 +386,9 @@ int32_t mxb_bank_set_state(mxb_bank* b, int32_t id, const double* values, int32_
             MXB_REQUIRE(fabs(h[v]) < 2147483648.0, MXB_ERR_INVALID, "mxb_bank_set_state: holdcount[%zu] = %g", v, h[v]);
             t[v] = (long long)h[v];
         }
-        MXB_CUDA(cudaMemcpy(b->env_holdcount, t.data(), sizeof(long long) * V, cudaMemcpyHostToDevice));
+        MXB_CUDA(cudaMemcpy(b->env_holdcount.get(), t.data(), sizeof(long long) * V, cudaMemcpyHostToDevice));
     } else {
-        int* d = id == MXB_S_ENV_FLAGS ? b->env_flags : b->dl_phase;
+        int* d = id == MXB_S_ENV_FLAGS ? b->env_flags.get() : b->dl_phase.get();
         MXB_REQUIRE(d, MXB_ERR_STATE, "mxb_bank_set_state: bank has no delay line");
         std::vector<int> t(V);
         for (size_t v = 0; v < V; ++v) {
@@ -422,20 +412,22 @@ int32_t mxb_bank_clone(mxb_bank* src, mxb_bank** out) {
     int rc = mxb_bank_create(src->ctx, &src->desc, &b);
     if (rc != MXB_OK) return rc;
     DeviceGuard g(src->ctx->device);
-    const size_t V = (size_t)src->V;
     cudaError_t e = cudaDeviceSynchronize();
-    auto cp = [&](void* d, const void* s, size_t bytes) { if (e == cudaSuccess && d && s) e = cudaMemcpy(d, s, bytes, cudaMemcpyDeviceToDevice); };
-    for (int i = 0; i < MXB_P_COUNT; ++i) { b->hp[i] = src->hp[i]; b->set_mask[i] = src->set_mask[i]; cp(b->dp[i], src->dp[i], sizeof(double) * V); }   // (an upload still in flight on the source is not part of its state yet)
-    cp(b->osc_out, src->osc_out, sizeof(double) * V);
-    cp(b->f0, src->f0, sizeof(double) * V); cp(b->f1, src->f1, sizeof(double) * V); cp(b->f2, src->f2, sizeof(double) * V);
-    for (int i = 0; i < 5; ++i) cp(b->cf[i], src->cf[i], sizeof(double) * V);
-    cp(b->env_amp, src->env_amp, sizeof(double) * V); cp(b->env_output, src->env_output, sizeof(double) * V);
-    cp(b->env_holdcount, src->env_holdcount, sizeof(long long) * V); cp(b->env_hold, src->env_hold, sizeof(long long) * V);
-    cp(b->env_flags, src->env_flags, sizeof(int) * V);
-    if (src->desc.delay_taps > 0) {
-        cp(b->dl_phase, src->dl_phase, sizeof(int) * V); cp(b->dl_size, src->dl_size, sizeof(int) * V); cp(b->dl_pos, src->dl_pos, sizeof(int) * V);
-        cp(b->ring, src->ring, sizeof(double) * dl_ring_doubles(V, src->desc.delay_taps));
+    // whole buffers; the two banks have the same description, so the same buffers of the same sizes
+    auto cp = [&](auto& d, const auto& s) {
+        if (e == cudaSuccess && d.get() && s.get()) e = cudaMemcpy(d.get(), s.get(), sizeof(*s.get()) * s.size(), cudaMemcpyDeviceToDevice);
+    };
+    for (int i = 0; i < MXB_P_COUNT; ++i) {     // the current parameter buffers (an upload still in flight on the source is not part of its state yet)
+        b->hp[i] = src->hp[i]; b->set_mask[i] = src->set_mask[i];
+        cp(b->dp_buf[i][0], src->dp_buf[i][src->dp_cur[i]]);
     }
+    cp(b->osc_out, src->osc_out);
+    cp(b->f0, src->f0); cp(b->f1, src->f1); cp(b->f2, src->f2);
+    for (int i = 0; i < 5; ++i) cp(b->cf[i], src->cf[i]);
+    cp(b->env_amp, src->env_amp); cp(b->env_output, src->env_output);
+    cp(b->env_holdcount, src->env_holdcount); cp(b->env_hold, src->env_hold); cp(b->env_flags, src->env_flags);
+    cp(b->dl_phase, src->dl_phase); cp(b->dl_size, src->dl_size); cp(b->dl_pos, src->dl_pos);
+    cp(b->ring, src->ring);
     if (e != cudaSuccess) { set_error("mxb_bank_clone: %s", cudaGetErrorString(e)); mxb_bank_destroy(b); return MXB_ERR_CUDA; }
     *out = b;
     return MXB_OK;
@@ -487,8 +479,6 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     const size_t V = (size_t)b->V;
     const size_t esz = out_dtype == MXB_F32 ? 4 : 8;
 
-    const int* d_on = trig_on; const int* d_off = trig_off;
-    void* d_out = out; double* d_mix = mix;
     if (cutoff_tv)
         MXB_REQUIRE(fk == MXB_FILT_LORES || fk == MXB_FILT_HIRES || fk == MXB_FILT_SVF, MXB_ERR_UNSUPPORTED,
                     "mxb_bank_process_mod: per-sample cutoff is built for lores / hires / maxiSVF");
@@ -496,42 +486,27 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
         MXB_REQUIRE(b->desc.delay_taps > 0, MXB_ERR_UNSUPPORTED, "mxb_bank_process_mod: delay_size_tv on a bank without a delay line");
     // per-sample parameters are control data: they live where the gates live
     const size_t nv = (size_t)n_frames * V;
-    auto stage = [&](const auto* src, auto** buf, size_t* len, const auto** dev) -> int {
-        *dev = src;
-        if (!src || !host_ctl) return MXB_OK;
-        const int rc = ensure(buf, len, nv, s);
-        if (rc != MXB_OK) return rc;
-        MXB_CUDA(cudaMemcpyAsync(*buf, src, sizeof(*src) * nv, cudaMemcpyHostToDevice, s));
-        *dev = *buf;
-        return MXB_OK;
-    };
     const double *d_fm, *d_cm, *d_ds;
     const unsigned char* d_tv;
-    int rc = stage(freq_tv, &b->fm_stage, &b->fm_stage_len, &d_fm);
-    if (rc == MXB_OK) rc = stage(cutoff_tv, &b->cm_stage, &b->cm_stage_len, &d_cm);
-    if (rc == MXB_OK) rc = stage(dsize_tv, &b->ds_stage, &b->ds_stage_len, &d_ds);
-    if (rc == MXB_OK) rc = stage(trig_tv, &b->tv_stage, &b->tv_stage_len, &d_tv);
+    const int *d_on, *d_off;
+    unsigned char* d_out;
+    double* d_mix;
+    int rc = stage_in(host_ctl, freq_tv, nv, b->fm_stage, s, &d_fm);
+    if (rc == MXB_OK) rc = stage_in(host_ctl, cutoff_tv, nv, b->cm_stage, s, &d_cm);
+    if (rc == MXB_OK) rc = stage_in(host_ctl, dsize_tv, nv, b->ds_stage, s, &d_ds);
+    if (rc == MXB_OK) rc = stage_in(host_ctl, trig_tv, nv, b->tv_stage, s, &d_tv);
+    if (rc == MXB_OK) rc = stage_in(host_ctl, trig_on, V, b->trig_on, s, &d_on);
+    if (rc == MXB_OK) rc = stage_in(host_ctl, trig_off, V, b->trig_off, s, &d_off);
+    if (rc == MXB_OK) rc = stage_out(host_out, (unsigned char*)out, nv * esz, b->out_stage, s, &d_out);
+    if (rc == MXB_OK) rc = stage_out(host_ctl, mix, (size_t)n_frames * 2, b->mix_dev, s, &d_mix);
     if (rc != MXB_OK) return rc;
-    if (host_ctl) {
-        if (trig_on) {
-            MXB_CUDA(cudaMemcpyAsync(b->trig_on, trig_on, sizeof(int) * V, cudaMemcpyHostToDevice, s));
-            MXB_CUDA(cudaMemcpyAsync(b->trig_off, trig_off, sizeof(int) * V, cudaMemcpyHostToDevice, s));
-            d_on = b->trig_on; d_off = b->trig_off;
-        }
-        if (out && host_out) {
-            rc = ensure(&b->out_stage, &b->out_stage_len, nv * esz, s);
-            if (rc != MXB_OK) return rc;
-            d_out = b->out_stage;
-        }
-        if (mix) d_mix = b->mix_dev;
-    }
 
     const int per_cta = kBankBlock * kBankVPT;
     const int grid = (int)((V + per_cta - 1) / per_cta);
     // warps that own at least one voice (warps past the end of the bank exit without writing partials)
     const int W = b->desc.delay_taps > 0 ? delay_bank_warps(b->V) : (int)((V + 32 * kBankVPT - 1) / (32 * kBankVPT));
     if (mix) {
-        rc = ensure(&b->partials, &b->partials_len, (size_t)b->desc.max_frames * 2 * (size_t)W, s);
+        rc = b->partials.grow((size_t)b->desc.max_frames * 2 * (size_t)W, s);
         if (rc != MXB_OK) return rc;
     }
 
@@ -544,7 +519,7 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
         MXB_CUDA(cudaEventRecord(b->ev_read[id][old], s));
         b->ev_read_set[id][old] = true;
         MXB_CUDA(cudaStreamWaitEvent(s, b->ev_up[id], 0));
-        b->dp_cur[id] ^= 1; b->dp[id] = b->dp_buf[id][b->dp_cur[id]]; b->dp_pending[id] = false;
+        b->dp_cur[id] ^= 1; b->dp[id] = b->dp_buf[id][b->dp_cur[id]].get(); b->dp_pending[id] = false;
     }
     BankArgs a;
     memset(&a, 0, sizeof(a));
@@ -555,15 +530,15 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     a.sr = (double)(size_t)b->ctx->sample_rate;
     for (int i = 0; i < 4; ++i) a.svf_mix[i] = b->desc.svf_mix[i];
     a.freq_tv = d_fm; a.cutoff_tv = d_cm; a.res = b->dp[MXB_P_RESONANCE];
-    a.freq = b->dp[MXB_P_FREQ]; a.duty = b->dp[MXB_P_DUTY]; a.pstart = b->dp[MXB_P_PHASOR_START]; a.pend = b->dp[MXB_P_PHASOR_END]; a.phase = b->dp[MXB_P_PHASE]; a.osc_out = b->osc_out;
-    a.f0 = b->f0; a.f1 = b->f1; a.f2 = b->f2;
-    for (int i = 0; i < 5; ++i) a.cf[i] = b->cf[i];
+    a.freq = b->dp[MXB_P_FREQ]; a.duty = b->dp[MXB_P_DUTY]; a.pstart = b->dp[MXB_P_PHASOR_START]; a.pend = b->dp[MXB_P_PHASOR_END]; a.phase = b->dp[MXB_P_PHASE]; a.osc_out = b->osc_out.get();
+    a.f0 = b->f0.get(); a.f1 = b->f1.get(); a.f2 = b->f2.get();
+    for (int i = 0; i < 5; ++i) a.cf[i] = b->cf[i].get();
     a.env_att = b->dp[MXB_P_ENV_ATTACK]; a.env_dec = b->dp[MXB_P_ENV_DECAY];
     a.env_sus = b->dp[MXB_P_ENV_SUSTAIN]; a.env_rel = b->dp[MXB_P_ENV_RELEASE];
-    a.env_hold = b->env_hold; a.env_amp = b->env_amp; a.env_output = b->env_output;
-    a.env_holdcount = b->env_holdcount; a.env_flags = b->env_flags;
+    a.env_hold = b->env_hold.get(); a.env_amp = b->env_amp.get(); a.env_output = b->env_output.get();
+    a.env_holdcount = b->env_holdcount.get(); a.env_flags = b->env_flags.get();
     a.trig_on = d_on; a.trig_off = d_off; a.trig_tv = d_tv;
-    a.out = d_out; a.pan = b->dp[MXB_P_PAN]; a.partials = b->partials;
+    a.out = d_out; a.pan = b->dp[MXB_P_PAN]; a.partials = b->partials.get();
 
     int osc_t = OSC_T_GENERIC;
     if (b->desc.osc_kind == MXB_OSC_SINEWAVE) osc_t = OSC_T_SINE;
@@ -576,9 +551,9 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
 
     if (b->desc.delay_taps > 0) {
         DelayArgs da;
-        da.phase = b->dl_phase; da.size = b->dl_size; da.feedback = b->dp[MXB_P_DELAY_FEEDBACK];
-        da.ring = b->ring; da.taps = b->desc.delay_taps;
-        da.from_position = b->desc.delay_mode == MXB_DELAY_FROM_POSITION ? 1 : 0; da.position = b->dl_pos;
+        da.phase = b->dl_phase.get(); da.size = b->dl_size.get(); da.feedback = b->dp[MXB_P_DELAY_FEEDBACK];
+        da.ring = b->ring.get(); da.taps = b->desc.delay_taps;
+        da.from_position = b->desc.delay_mode == MXB_DELAY_FROM_POSITION ? 1 : 0; da.position = b->dl_pos.get();
         da.size_tv = d_ds;
         rc = launch_delay_bank(a, da, fk, svf_lp, env, out != nullptr, mix != nullptr, s);
         if (rc != MXB_OK) return rc;
@@ -597,7 +572,7 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     }
     b->launches += 1;
     if (mix) {
-        rc = mix_bus_reduce(b->ex, b->partials, W, n_frames, d_mix, s);
+        rc = mix_bus_reduce(b->ex, b->partials.get(), W, n_frames, d_mix, s);
         if (rc != MXB_OK) return rc;
         b->launches += 1;
     }

@@ -12,6 +12,8 @@
 #include <stdarg.h>
 #include <string.h>
 #include <stdlib.h>
+#include <memory>
+#include <utility>
 #include <vector>
 
 #include "../../include/maxib200.h"
@@ -55,29 +57,74 @@ struct DeviceGuard {
     ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
+// One device allocation (plain cudaMalloc), freed when the buffer is destroyed. Empty until alloc / grow / upload.
 template <class T>
-inline int dev_alloc(T** p, size_t n, bool zero = true) {
-    void* q = nullptr;
-    cudaError_t e = cudaMalloc(&q, sizeof(T) * (n ? n : 1));
-    if (e != cudaSuccess) { set_error("cudaMalloc(%zu bytes): %s", sizeof(T) * n, cudaGetErrorString(e)); return MXB_ERR_ALLOC; }
-    if (zero) {
-        e = cudaMemset(q, 0, sizeof(T) * (n ? n : 1));
-        if (e != cudaSuccess) { set_error("cudaMemset: %s", cudaGetErrorString(e)); cudaFree(q); return MXB_ERR_CUDA; }
+class DevBuf {
+public:
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p_, o.p_); std::swap(n_, o.n_); return *this; }
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p_) cudaFree(p_); }
+
+    // max(n, 1) elements, zero-filled unless `zero` is false; replaces any earlier allocation
+    int alloc(size_t n, bool zero = true) {
+        release();
+        void* q = nullptr;
+        cudaError_t e = cudaMalloc(&q, sizeof(T) * (n ? n : 1));
+        if (e != cudaSuccess) { set_error("cudaMalloc(%zu bytes): %s", sizeof(T) * n, cudaGetErrorString(e)); return MXB_ERR_ALLOC; }
+        if (zero) {
+            e = cudaMemset(q, 0, sizeof(T) * (n ? n : 1));
+            if (e != cudaSuccess) { set_error("cudaMemset: %s", cudaGetErrorString(e)); cudaFree(q); return MXB_ERR_CUDA; }
+        }
+        p_ = (T*)q; n_ = n;
+        return MXB_OK;
     }
-    *p = (T*)q;
+    // Grows a staging buffer to at least `n` elements (contents not kept). Work queued on `s` may still read the old
+    // buffer, so `s` is synchronised before it is freed.
+    int grow(size_t n, cudaStream_t s) {
+        if (n <= n_) return MXB_OK;
+        MXB_CUDA(cudaStreamSynchronize(s));
+        return alloc(n, false);
+    }
+    int upload(const std::vector<T>& v) {
+        const int rc = alloc(v.size(), false);
+        if (rc != MXB_OK) return rc;
+        MXB_CUDA(cudaMemcpy(p_, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice));
+        return MXB_OK;
+    }
+    T* get() const { return p_; }
+    size_t size() const { return n_; }
+
+private:
+    void release() { if (p_) cudaFree(p_); p_ = nullptr; n_ = 0; }
+    T* p_ = nullptr;
+    size_t n_ = 0;       // elements asked for
+};
+
+// MXB_MEM_HOST data reaches a kernel through a staging buffer of the handle. stage_in: with `host` set, copies `n`
+// elements of `src` into `buf` on `s` and points `*dev` at the copy; otherwise (or for a NULL `src`) `*dev` is `src`.
+template <class T>
+int stage_in(bool host, const T* src, size_t n, DevBuf<T>& buf, cudaStream_t s, const T** dev) {
+    *dev = src;
+    if (!host || !src) return MXB_OK;
+    const int rc = buf.grow(n, s);
+    if (rc != MXB_OK) return rc;
+    MXB_CUDA(cudaMemcpyAsync(buf.get(), src, sizeof(T) * n, cudaMemcpyHostToDevice, s));
+    *dev = buf.get();
     return MXB_OK;
 }
-
-// Grows a staging buffer to at least `need` elements (contents not kept). Work queued on `s` may still read the old
-// buffer, so `s` is synchronised before it is freed.
+// stage_out: with `host` set, points `*dev` at `buf` grown to `n` elements (the caller copies the results back to
+// `dst`); otherwise (or for a NULL `dst`) `*dev` is `dst`.
 template <class T>
-inline int ensure(T** p, size_t* len, size_t need, cudaStream_t s) {
-    if (need <= *len) return MXB_OK;
-    MXB_CUDA(cudaStreamSynchronize(s));
-    cudaFree(*p); *p = nullptr; *len = 0;
-    const int rc = dev_alloc(p, need, false);
-    if (rc == MXB_OK) *len = need;
-    return rc;
+int stage_out(bool host, T* dst, size_t n, DevBuf<T>& buf, cudaStream_t s, T** dev) {
+    *dev = dst;
+    if (!host || !dst) return MXB_OK;
+    const int rc = buf.grow(n, s);
+    if (rc != MXB_OK) return rc;
+    *dev = buf.get();
+    return MXB_OK;
 }
 
 }  // namespace mxb
@@ -88,7 +135,7 @@ struct mxb_ctx {
     int sm_count;
     int cc_major, cc_minor;
     int smem_optin;          // cudaDevAttrMaxSharedMemoryPerBlockOptin: the most shared memory one CTA may opt in to
-    double* d_sine;          // sineBuffer[514] ++ transition[1001] of the reference (mxb_ctx_set_tables), or NULL
+    mxb::DevBuf<double> d_sine;      // sineBuffer[514] ++ transition[1001] of the reference (mxb_ctx_set_tables), or empty
     double sine_before;
 };
 #endif  // __CUDACC_RTC__

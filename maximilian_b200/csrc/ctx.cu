@@ -47,13 +47,14 @@ int32_t mxb_ctx_create(int32_t device, int32_t sample_rate, mxb_ctx** out) {
     c->cc_major = prop.major;
     c->cc_minor = prop.minor;
     c->smem_optin = smem_optin;
-    c->d_sine = nullptr; c->sine_before = 0.0;
+    c->sine_before = 0.0;
     *out = c;
     return MXB_OK;
 }
 
 int32_t mxb_ctx_destroy(mxb_ctx* ctx) {
-    if (ctx && ctx->d_sine) { mxb::DeviceGuard g(ctx->device); cudaFree(ctx->d_sine); }
+    if (!ctx) return MXB_OK;
+    mxb::DeviceGuard g(ctx->device);
     delete ctx;
     return MXB_OK;
 }

@@ -42,13 +42,18 @@ struct mxb_exchange {
     mxb_ctx* ctx;
     int rank, world, max_doubles;
     size_t flags_bytes, slot_bytes;           // slot = world * max_doubles doubles, 128-byte multiple
-    unsigned char* local;                     // cudaMalloc'ed: flags + 2 slots
+    mxb::DevBuf<unsigned char> local;         // flags + 2 slots; a plain cudaMalloc allocation, exportable with cudaIpcGetMemHandle
     unsigned char* peers[mxb::kExchMaxWorld]; // cudaIpcOpenMemHandle'd (own entry = local)
     bool connected;
     unsigned long long seq;                   // calls so far
-    unsigned int* ticket;
-    unsigned int* status;                     // device word, see ExchDev::status
+    mxb::DevBuf<unsigned int> ticket;
+    mxb::DevBuf<unsigned int> status;         // device word, see ExchDev::status
     unsigned long long timeout_ns;            // default 5 s; MXB_EXCHANGE_TIMEOUT_MS overrides
+
+    ~mxb_exchange() {
+        for (int r = 0; r < world; ++r)
+            if (r != rank && peers[r]) cudaIpcCloseMemHandle(peers[r]);
+    }
 };
 
 namespace {
@@ -132,13 +137,13 @@ ExchDev exchange_next(mxb_exchange* ex) {
     ExchDev d;
     memset(&d, 0, sizeof(d));
     const size_t slot_off = ex->flags_bytes + (size_t)(ex->seq & 1) * ex->slot_bytes;
-    d.rank = ex->rank; d.world = ex->world; d.stride = ex->max_doubles; d.seq1 = ex->seq + 1; d.ticket = ex->ticket; d.status = ex->status; d.timeout_ns = ex->timeout_ns;
+    d.rank = ex->rank; d.world = ex->world; d.stride = ex->max_doubles; d.seq1 = ex->seq + 1; d.ticket = ex->ticket.get(); d.status = ex->status.get(); d.timeout_ns = ex->timeout_ns;
     for (int r = 0; r < ex->world; ++r) {
         d.dst_flag[r] = (unsigned long long*)(ex->peers[r] + (size_t)ex->rank * kExchFlagBytes);
         d.dst_payload[r] = (double*)(ex->peers[r] + slot_off) + (size_t)ex->rank * (size_t)ex->max_doubles;
     }
-    d.src_flags = (const unsigned long long*)ex->local;
-    d.src_payload = (const double*)(ex->local + slot_off);
+    d.src_flags = (const unsigned long long*)ex->local.get();
+    d.src_payload = (const double*)(ex->local.get() + slot_off);
     ex->seq += 1;
     return d;
 }
@@ -186,31 +191,23 @@ int32_t mxb_exchange_create(mxb_ctx* ctx, int32_t rank, int32_t world, int32_t m
     MXB_REQUIRE(world >= 1 && world <= kExchMaxWorld && rank >= 0 && rank < world, MXB_ERR_INVALID, "mxb_exchange_create: rank %d of %d", rank, world);
     MXB_REQUIRE(max_doubles > 0, MXB_ERR_INVALID, "mxb_exchange_create: max_doubles %d", max_doubles);
     DeviceGuard g(ctx->device);
-    mxb_exchange* ex = new (std::nothrow) mxb_exchange();
+    std::unique_ptr<mxb_exchange> ex(new (std::nothrow) mxb_exchange());
     MXB_REQUIRE(ex, MXB_ERR_ALLOC, "mxb_exchange_create: out of host memory");
-    memset(ex, 0, sizeof(*ex));
     ex->ctx = ctx; ex->rank = rank; ex->world = world; ex->max_doubles = max_doubles;
     ex->flags_bytes = (size_t)kExchMaxWorld * kExchFlagBytes;
     ex->slot_bytes = (sizeof(double) * (size_t)max_doubles * (size_t)world + 127) & ~(size_t)127;
-    const size_t total = ex->flags_bytes + 2 * ex->slot_bytes;
-    void* p = nullptr;
-    cudaError_t e = cudaMalloc(&p, total);                   // plain cudaMalloc: exportable with cudaIpcGetMemHandle
-    if (e != cudaSuccess) { set_error("mxb_exchange_create: cudaMalloc: %s", cudaGetErrorString(e)); delete ex; return MXB_ERR_ALLOC; }
-    ex->local = (unsigned char*)p;
-    e = cudaMemset(p, 0, total);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&ex->ticket, sizeof(unsigned int));
-    if (e == cudaSuccess) e = cudaMemset(ex->ticket, 0, sizeof(unsigned int));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&ex->status, sizeof(unsigned int));
-    if (e == cudaSuccess) e = cudaMemset(ex->status, 0, sizeof(unsigned int));
+    int rc = ex->local.alloc(ex->flags_bytes + 2 * ex->slot_bytes);      // zero-filled, like ticket and status
+    if (rc == MXB_OK) rc = ex->ticket.alloc(1);
+    if (rc == MXB_OK) rc = ex->status.alloc(1);
+    if (rc != MXB_OK) return rc;
     {   // a dead peer must not hang the others: the flag wait is bounded (the kernel then reports through `status`)
         const char* t = getenv("MXB_EXCHANGE_TIMEOUT_MS");
         const double ms = t ? atof(t) : 5000.0;
         ex->timeout_ns = (unsigned long long)((ms > 0.0 ? ms : 5000.0) * 1e6);
     }
-    if (e != cudaSuccess) { set_error("mxb_exchange_create: %s", cudaGetErrorString(e)); cudaFree(p); delete ex; return MXB_ERR_CUDA; }
-    ex->peers[rank] = ex->local;
+    ex->peers[rank] = ex->local.get();
     ex->connected = (world == 1);
-    *out = ex;
+    *out = ex.release();
     return MXB_OK;
 }
 
@@ -219,7 +216,7 @@ int32_t mxb_exchange_local_handle(mxb_exchange* ex, void* handle, int32_t handle
     MXB_REQUIRE(handle_bytes >= (int32_t)sizeof(cudaIpcMemHandle_t), MXB_ERR_INVALID, "mxb_exchange_local_handle: need %zu bytes", sizeof(cudaIpcMemHandle_t));
     DeviceGuard g(ex->ctx->device);
     cudaIpcMemHandle_t h;
-    MXB_CUDA(cudaIpcGetMemHandle(&h, ex->local));
+    MXB_CUDA(cudaIpcGetMemHandle(&h, ex->local.get()));
     memcpy(handle, &h, sizeof(h));
     return MXB_OK;
 }
@@ -244,7 +241,7 @@ int32_t mxb_exchange_status(mxb_exchange* ex, int32_t* timed_out_ranks) {
     MXB_REQUIRE(ex && timed_out_ranks, MXB_ERR_INVALID, "mxb_exchange_status: NULL argument");
     DeviceGuard g(ex->ctx->device);
     unsigned int m = 0;
-    MXB_CUDA(cudaMemcpy(&m, ex->status, sizeof(m), cudaMemcpyDeviceToHost));      // synchronises with the kernels that may set it
+    MXB_CUDA(cudaMemcpy(&m, ex->status.get(), sizeof(m), cudaMemcpyDeviceToHost));      // synchronises with the kernels that may set it
     *timed_out_ranks = (int32_t)m;
     return MXB_OK;
 }
@@ -253,9 +250,6 @@ int32_t mxb_exchange_destroy(mxb_exchange* ex) {
     if (!ex) return MXB_OK;
     DeviceGuard g(ex->ctx->device);
     cudaDeviceSynchronize();
-    for (int r = 0; r < ex->world; ++r)
-        if (r != ex->rank && ex->peers[r]) cudaIpcCloseMemHandle(ex->peers[r]);
-    cudaFree(ex->local); cudaFree(ex->ticket); cudaFree(ex->status);
     delete ex;
     return MXB_OK;
 }

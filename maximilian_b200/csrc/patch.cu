@@ -282,11 +282,11 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
         if (patch_stage_rings(g.op)) { MXB_REQUIRE(d->delay_taps > 0, MXB_ERR_INVALID, "%s: stage %d needs delay_taps > 0", who, i); n_rings += patch_stage_rings(g.op); }
         n_state += patch_state_slots(g.op);
     }
-    if (tables) MXB_REQUIRE(ctx->d_sine, MXB_ERR_STATE, "%s: sinebuf / sinebuf4 / sawn need the reference's tables: call mxb_ctx_set_tables first", who);
+    if (tables) MXB_REQUIRE(ctx->d_sine.get(), MXB_ERR_STATE, "%s: sinebuf / sinebuf4 / sawn need the reference's tables: call mxb_ctx_set_tables first", who);
     const size_t per_thread = (size_t)(kMaxRegs + d->n_params + n_state);
     MXB_REQUIRE(per_thread * 8 * kPatchThreads <= 200 * 1024, MXB_ERR_UNSUPPORTED, "%s: %zu doubles of registers, parameters and state per voice do not fit shared memory", who, per_thread);
     DeviceGuard g(ctx->device);
-    mxb_patch* p = new (std::nothrow) mxb_patch();
+    std::unique_ptr<mxb_patch> p(new (std::nothrow) mxb_patch());
     MXB_REQUIRE(p, MXB_ERR_ALLOC, "%s: out of host memory", who);
     p->ctx = ctx; p->V = d->voices; p->n_stages = d->n_stages; p->n_params = d->n_params; p->n_consts = d->n_consts; p->n_inputs = d->n_inputs;
     p->max_frames = d->max_frames; p->taps = d->delay_taps; p->n_state = n_state; p->n_rings = n_rings;
@@ -307,26 +307,27 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
         eg_segments(shapes[k], (double)(size_t)ctx->sample_rate, p->eg[k]);
     }
     const size_t V = (size_t)p->V;
-#define TRY(x) do { rc = (x); if (rc != MXB_OK) { mxb_patch_destroy(p); return rc; } } while (0)
-    TRY(dev_alloc(&p->d_stages, (size_t)d->n_stages)); TRY(dev_alloc(&p->d_state_base, (size_t)d->n_stages)); TRY(dev_alloc(&p->d_ring_of, (size_t)d->n_stages));
-    TRY(dev_alloc(&p->d_consts, (size_t)kMaxConsts));
-    TRY(dev_alloc(&p->params, (size_t)(d->n_params ? d->n_params : 1) * V));
-    TRY(dev_alloc(&p->state, (size_t)(n_state ? n_state : 1) * V));
-    if (n_rings) TRY(dev_alloc(&p->rings, (size_t)n_rings * (size_t)p->taps * V));
-    TRY(dev_alloc(&p->mix_dev, (size_t)p->max_frames * 2));
-    cudaError_t e = cudaMemcpy(p->d_stages, p->stages.data(), sizeof(mxb_stage) * d->n_stages, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_state_base, p->state_base.data(), sizeof(int) * d->n_stages, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_ring_of, p->ring_of.data(), sizeof(int) * d->n_stages, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && d->n_consts) e = cudaMemcpy(p->d_consts, d->consts, sizeof(double) * d->n_consts, cudaMemcpyHostToDevice);
+    if (rc == MXB_OK) rc = p->d_stages.alloc((size_t)d->n_stages);
+    if (rc == MXB_OK) rc = p->d_state_base.alloc((size_t)d->n_stages);
+    if (rc == MXB_OK) rc = p->d_ring_of.alloc((size_t)d->n_stages);
+    if (rc == MXB_OK) rc = p->d_consts.alloc((size_t)kMaxConsts);
+    if (rc == MXB_OK) rc = p->params.alloc((size_t)(d->n_params ? d->n_params : 1) * V);
+    if (rc == MXB_OK) rc = p->state.alloc((size_t)(n_state ? n_state : 1) * V);
+    if (rc == MXB_OK && n_rings) rc = p->rings.alloc((size_t)n_rings * (size_t)p->taps * V);
+    if (rc == MXB_OK) rc = p->mix_dev.alloc((size_t)p->max_frames * 2);
+    if (rc != MXB_OK) return rc;
+    cudaError_t e = cudaMemcpy(p->d_stages.get(), p->stages.data(), sizeof(mxb_stage) * d->n_stages, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(p->d_state_base.get(), p->state_base.data(), sizeof(int) * d->n_stages, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(p->d_ring_of.get(), p->ring_of.data(), sizeof(int) * d->n_stages, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && d->n_consts) e = cudaMemcpy(p->d_consts.get(), d->consts, sizeof(double) * d->n_consts, cudaMemcpyHostToDevice);
     for (int i = 0; i < d->n_stages && e == cudaSuccess; ++i)
         for (int k = 0; k < patch_state_slots(p->stages[i].op) && e == cudaSuccess; ++k)
-            if (patch_state_init(p->stages[i].op, k) != 0.0) {                 // dev_alloc zeroed the others
+            if (patch_state_init(p->stages[i].op, k) != 0.0) {                 // alloc zeroed the others
                 const std::vector<double> col(V, patch_state_init(p->stages[i].op, k));
-                e = cudaMemcpy(p->state + (size_t)(p->state_base[i] + k) * V, col.data(), sizeof(double) * V, cudaMemcpyHostToDevice);
+                e = cudaMemcpy(p->state.get() + (size_t)(p->state_base[i] + k) * V, col.data(), sizeof(double) * V, cudaMemcpyHostToDevice);
             }
-    if (e != cudaSuccess) { set_error("%s: %s", who, cudaGetErrorString(e)); mxb_patch_destroy(p); return MXB_ERR_CUDA; }
-#undef TRY
-    *out = p;
+    if (e != cudaSuccess) { set_error("%s: %s", who, cudaGetErrorString(e)); return MXB_ERR_CUDA; }
+    *out = p.release();
     return MXB_OK;
 }
 
@@ -337,9 +338,9 @@ extern "C" {
 int32_t mxb_ctx_set_tables(mxb_ctx* ctx, const double* sine514, const double* transition1001, double sine_before) {
     MXB_REQUIRE(ctx && sine514 && transition1001, MXB_ERR_INVALID, "mxb_ctx_set_tables: NULL argument");
     DeviceGuard g(ctx->device);
-    if (!ctx->d_sine) { int rc = dev_alloc(&ctx->d_sine, 514 + 1001); if (rc != MXB_OK) return rc; }
-    MXB_CUDA(cudaMemcpy(ctx->d_sine, sine514, sizeof(double) * 514, cudaMemcpyHostToDevice));
-    MXB_CUDA(cudaMemcpy(ctx->d_sine + 514, transition1001, sizeof(double) * 1001, cudaMemcpyHostToDevice));
+    if (!ctx->d_sine.get()) { int rc = ctx->d_sine.alloc(514 + 1001); if (rc != MXB_OK) return rc; }
+    MXB_CUDA(cudaMemcpy(ctx->d_sine.get(), sine514, sizeof(double) * 514, cudaMemcpyHostToDevice));
+    MXB_CUDA(cudaMemcpy(ctx->d_sine.get() + 514, transition1001, sizeof(double) * 1001, cudaMemcpyHostToDevice));
     ctx->sine_before = sine_before;
     return MXB_OK;
 }
@@ -367,10 +368,6 @@ int32_t mxb_patch_destroy(mxb_patch* p) {
     if (!p) return MXB_OK;
     DeviceGuard g(p->ctx->device);
     cudaDeviceSynchronize();
-    patch_fused_free(p);
-    cudaFree(p->d_stages); cudaFree(p->d_state_base); cudaFree(p->d_ring_of); cudaFree(p->d_consts);
-    cudaFree(p->params); cudaFree(p->state); cudaFree(p->rings); cudaFree(p->out_stage); cudaFree(p->partials); cudaFree(p->mix_dev);
-    for (auto q : p->in_stage) cudaFree(q);
     delete p;
     return MXB_OK;
 }
@@ -380,7 +377,7 @@ int32_t mxb_patch_set_param(mxb_patch* p, int32_t j, const double* values, int32
     MXB_REQUIRE(j >= 0 && j < p->n_params, MXB_ERR_INVALID, "mxb_patch_set_param: parameter %d of %d", j, p->n_params);
     MXB_REQUIRE(mem == MXB_MEM_HOST || mem == MXB_MEM_DEVICE, MXB_ERR_INVALID, "mxb_patch_set_param: mem %d", mem);
     DeviceGuard g(p->ctx->device);
-    MXB_CUDA(cudaMemcpy(p->params + (size_t)j * p->V, values, sizeof(double) * (size_t)p->V, mem == MXB_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice));
+    MXB_CUDA(cudaMemcpy(p->params.get() + (size_t)j * p->V, values, sizeof(double) * (size_t)p->V, mem == MXB_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice));
     return MXB_OK;
 }
 
@@ -388,7 +385,7 @@ static int32_t patch_state_ptr(mxb_patch* p, int32_t stage, int32_t slot, double
     MXB_REQUIRE(p, MXB_ERR_INVALID, "%s: NULL patch", who);
     MXB_REQUIRE(stage >= 0 && stage < p->n_stages, MXB_ERR_INVALID, "%s: stage %d of %d", who, stage, p->n_stages);
     MXB_REQUIRE(slot >= 0 && slot < patch_state_slots(p->stages[stage].op), MXB_ERR_INVALID, "%s: stage %d has %d state slots, not %d", who, stage, patch_state_slots(p->stages[stage].op), slot);
-    *ptr = p->state + (size_t)(p->state_base[stage] + slot) * p->V;
+    *ptr = p->state.get() + (size_t)(p->state_base[stage] + slot) * p->V;
     return MXB_OK;
 }
 
@@ -417,7 +414,7 @@ int32_t mxb_patch_get_ring(mxb_patch* p, int32_t stage, int32_t voice, double* d
     MXB_REQUIRE(stage >= 0 && stage < p->n_stages && p->ring_of[stage] >= 0, MXB_ERR_INVALID, "mxb_patch_get_ring: stage %d has no delay line", stage);
     MXB_REQUIRE(voice >= 0 && voice < p->V && n >= 0 && n <= p->taps * patch_stage_rings(p->stages[stage].op), MXB_ERR_INVALID, "mxb_patch_get_ring: voice %d n %d", voice, n);
     DeviceGuard g(p->ctx->device);
-    const double* src = p->rings + (size_t)p->ring_of[stage] * (size_t)p->taps * (size_t)p->V + (size_t)voice;
+    const double* src = p->rings.get() + (size_t)p->ring_of[stage] * (size_t)p->taps * (size_t)p->V + (size_t)voice;
     if (n) MXB_CUDA(cudaMemcpy2D(dst, sizeof(double), src, sizeof(double) * (size_t)p->V, sizeof(double), (size_t)n,
                                  mem == MXB_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice));
     return MXB_OK;
@@ -472,39 +469,32 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
     const size_t V = (size_t)p->V, nb = sizeof(double) * (size_t)n_frames * V;
     PatchArgs a;
     memset(&a, 0, sizeof(a));
-    double* d_out = out; double* d_mix = mix;
+    const bool host = mem == MXB_MEM_HOST;
     for (int i = 0; i < p->n_inputs; ++i) {
-        a.inputs[i] = inputs[i];
         a.in_kind[i] = (unsigned char)p->in_type[i];
-        if (mem == MXB_MEM_HOST) {
-            const size_t nb = patch_input_bytes(p->in_type[i], (size_t)n_frames, V);
-            const int rc = ensure(&p->in_stage[i], &p->in_stage_len[i], nb, s);
-            if (rc != MXB_OK) return rc;
-            MXB_CUDA(cudaMemcpyAsync(p->in_stage[i], inputs[i], nb, cudaMemcpyHostToDevice, s));
-            a.inputs[i] = p->in_stage[i];
-        }
+        const unsigned char* d_in;
+        const int rc = stage_in(host, (const unsigned char*)inputs[i], patch_input_bytes(p->in_type[i], (size_t)n_frames, V), p->in_stage[i], s, &d_in);
+        if (rc != MXB_OK) return rc;
+        a.inputs[i] = d_in;
     }
-    if (mem == MXB_MEM_HOST) {
-        if (out) {
-            const int rc = ensure(&p->out_stage, &p->out_stage_len, (size_t)n_frames * V, s);
-            if (rc != MXB_OK) return rc;
-            d_out = p->out_stage;
-        }
-        if (mix) d_mix = p->mix_dev;
-    }
+    double *d_out, *d_mix;
+    int rc = stage_out(host, out, (size_t)n_frames * V, p->out_stage, s, &d_out);
+    if (rc == MXB_OK) rc = stage_out(host, mix, (size_t)n_frames * 2, p->mix_dev, s, &d_mix);
+    if (rc != MXB_OK) return rc;
     const int grid = (int)((V + kPatchThreads - 1) / kPatchThreads);
     const int W = grid * (kPatchThreads / 32);
-    if (mix) { const int rc = ensure(&p->partials, &p->partials_len, (size_t)p->max_frames * 2 * (size_t)W, s); if (rc != MXB_OK) return rc; }
+    if (mix) { rc = p->partials.grow((size_t)p->max_frames * 2 * (size_t)W, s); if (rc != MXB_OK) return rc; }
     a.V = p->V; a.n_frames = n_frames; a.n_stages = p->n_stages; a.n_params = p->n_params; a.n_state = p->n_state; a.W = W; a.taps = p->taps;
     a.sr = (double)(size_t)p->ctx->sample_rate;
-    a.stages = p->d_stages; a.state_base = p->d_state_base; a.ring_of = p->d_ring_of; a.consts = p->d_consts;
-    a.params = p->params; a.state = p->state; a.out = d_out; a.partials = mix ? p->partials : nullptr; a.rings = p->rings;
-    a.sine = p->ctx->d_sine; a.transition = p->ctx->d_sine ? p->ctx->d_sine + 514 : nullptr; a.sine_before = p->ctx->sine_before;
+    a.stages = p->d_stages.get(); a.state_base = p->d_state_base.get(); a.ring_of = p->d_ring_of.get(); a.consts = p->d_consts.get();
+    a.params = p->params.get(); a.state = p->state.get(); a.out = d_out; a.partials = mix ? p->partials.get() : nullptr; a.rings = p->rings.get();
+    const double* sine = p->ctx->d_sine.get();
+    a.sine = sine; a.transition = sine ? sine + 514 : nullptr; a.sine_before = p->ctx->sine_before;
     memcpy(a.eg_n, p->eg_n, sizeof(a.eg_n)); memcpy(a.eg_loop, p->eg_loop, sizeof(a.eg_loop)); memcpy(a.eg_retrigger, p->eg_retrigger, sizeof(a.eg_retrigger));
     memcpy(a.eg, p->eg, sizeof(a.eg));
     if (p->mode == MXB_PATCH_FUSED) {
         // the kernel generated for this stage list (patch_fuse.cu): compiled on first use, then launched like any other
-        int rc = patch_fused_load(p);
+        rc = patch_fused_load(p);
         if (rc == MXB_OK) rc = patch_fused_launch(p, a, grid, s);
         if (rc != MXB_OK) return rc;
     } else {
@@ -516,11 +506,11 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
     }
     p->launches += 1;
     if (mix) {
-        const int rc = mix_bus_reduce(p->ex, p->partials, W, n_frames, d_mix, s);
+        rc = mix_bus_reduce(p->ex, p->partials.get(), W, n_frames, d_mix, s);
         if (rc != MXB_OK) return rc;
         p->launches += 1;
     }
-    if (mem == MXB_MEM_HOST) {
+    if (host) {
         if (out) MXB_CUDA(cudaMemcpyAsync(out, d_out, nb, cudaMemcpyDeviceToHost, s));
         if (mix) MXB_CUDA(cudaMemcpyAsync(mix, d_mix, sizeof(double) * (size_t)n_frames * 2, cudaMemcpyDeviceToHost, s));
         MXB_CUDA(cudaStreamSynchronize(s));

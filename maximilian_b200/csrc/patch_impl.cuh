@@ -324,19 +324,17 @@ struct mxb_patch {
     std::vector<mxb_stage> stages;
     std::vector<int> state_base, ring_of;
     std::vector<double> consts;
-    mxb_stage* d_stages; int* d_state_base; int* d_ring_of; double* d_consts;
-    double* params; double* state; double* rings;
-    unsigned char* in_stage[mxb::kMaxInputs]; size_t in_stage_len[mxb::kMaxInputs];      // staging for MXB_MEM_HOST input streams (bytes)
+    mxb::DevBuf<mxb_stage> d_stages; mxb::DevBuf<int> d_state_base, d_ring_of; mxb::DevBuf<double> d_consts;
+    mxb::DevBuf<double> params, state, rings;
+    mxb::DevBuf<unsigned char> in_stage[mxb::kMaxInputs];      // staging for MXB_MEM_HOST input streams (bytes)
     int in_type[mxb::kMaxInputs];
-    double* out_stage; size_t out_stage_len;
-    double* partials; size_t partials_len;
-    double* mix_dev;
+    mxb::DevBuf<double> out_stage, partials, mix_dev;
     int n_shapes;          // maxiEnvGen shapes; ENVGEN stage kinds index them
     int eg_n[mxb::kMaxEgShapes], eg_loop[mxb::kMaxEgShapes], eg_retrigger[mxb::kMaxEgShapes];
     mxb::EgStage eg[mxb::kMaxEgShapes][mxb::kMaxEg];
     int64_t launches;
     int mode;              // MXB_PATCH_INTERPRET | MXB_PATCH_FUSED
-    mxb_fused* fused;      // compiled on the first fused launch
+    mxb_fused* fused;      // compiled on the first fused launch; owned by the module cache, which outlives the patch
     mxb_exchange* ex;      // peer-memory mix exchange (multi-GPU), or NULL
 };
 
@@ -347,6 +345,5 @@ std::string patch_generate_source(const mxb_stage* stages, int n_stages, int n_p
 int patch_compile(const std::string& src, std::vector<char>& cubin);
 int patch_fused_load(mxb_patch* p);                                   // generate + compile + load, once
 int patch_fused_launch(mxb_patch* p, const PatchArgs& a, int grid, cudaStream_t s);
-void patch_fused_free(mxb_patch* p);
 }  // namespace mxb
 #endif
