@@ -462,3 +462,93 @@ def test_per_sample_analysis_resynthesis_idiom(port, reference):
     z = np.zeros((1, 1, bins), dtype=np.float32)
     oy = port.Istft(1, n, hop, kind="port").process(np.concatenate([z, o["mags"][:, :K - 1]], axis=1), np.concatenate([z, o["phases"][:, :K - 1]], axis=1))
     assert same(y, np.ascontiguousarray(oy[0, :N]), equal_nan=False)
+
+
+# The corners the bank matrix (tests/bank_matrix.py) feeds the GPU banks, with the port pinned to the reference there first.
+FM_OUTSIDE_AUDIO = (0.0, -300.0, 2.0 ** -70, 2.0 ** 61, 72000.0, np.inf, np.nan)
+
+
+def _fm_outside_audio(V, B, blk, moderate=False):
+    """fm_frequencies() with, on chosen samples, every frequency outside the audio range (moderate: only those that keep a
+    sinewave's phase finite and small), on single voices and on all voices at once"""
+    f = fm_frequencies(V, B, blk)
+    vals = FM_OUTSIDE_AUDIO[:2] + FM_OUTSIDE_AUDIO[2:3] + FM_OUTSIDE_AUDIO[4:5] if moderate else FM_OUTSIDE_AUDIO
+    for k, c in enumerate(vals):
+        f[7 * k + 3, k % V] = c
+        f[7 * k + 5, (k + 1) % V] = c
+    f[B // 2, :] = 0.0
+    return f
+
+
+@pytest.mark.parametrize("osc", ["saw", "phasor", "square", "pulse", "impulse", "triangle", "phasorbetween", "sinewave", "coswave"])
+def test_fm_outside_the_audio_range_bit_exact(port, reference, osc):
+    V, B = 9, 64
+    p = W.voice_params(V, seed=35)
+    a, b = _pair(port, reference, V, osc=osc, filt="none")
+    _configure(a, "none", p); _configure(b, "none", p)
+    for blk in range(2):
+        f = _fm_outside_audio(V, B, blk, moderate=osc in ("sinewave", "coswave"))
+        oa, ma = a.process(B, freq_tv=f, want_mix=True); ob, mb = b.process(B, freq_tv=f, want_mix=True)
+        assert _same(oa, ob) and _same(ma, mb), blk
+        for s in ("phase", "osc_output"):
+            assert _same(a.get(s), b.get(s)), (blk, s)
+
+
+@pytest.mark.parametrize("filt", ["lores", "hires", "svf"])
+def test_cutoff_outside_the_clamp_bit_exact(port, reference, filt):
+    """per-sample cutoffs below the lores / hires clamp of 10 Hz, at and above the sample rate (lores / hires: clamped to sr, where
+    the design divides 0 by 0), SVF cutoffs at and above Nyquist and above the sample rate; resonances below 1"""
+    V, B = 8, 96
+    p = W.voice_params(V, seed=36)
+    p["q_lores"][:2] = (0.5, 0.0)
+    a, b = _pair(port, reference, V, osc="saw", filt=filt)
+    _configure(a, filt, p); _configure(b, filt, p)
+    for blk in range(2):
+        cu = cutoff_sweeps(V, B, blk)
+        cu[3, :4] = (5.0, 0.0, -100.0, 9.999)
+        cu[40, 4], cu[41, 5] = 24000.0, 30000.0
+        cu[60, 6] = 60000.0
+        if blk == 1:
+            cu[B - 1, 6], cu[B - 1, 7] = 48000.0, 96000.0
+        oa, ma = a.process(B, cutoff_tv=cu, want_mix=True); ob, mb = b.process(B, cutoff_tv=cu, want_mix=True)
+        assert _same(oa, ob) and _same(ma, mb), blk
+        for s in ("filt0", "filt1", "filt2"):
+            assert _same(a.get(s), b.get(s)), (blk, s)
+
+
+@pytest.mark.parametrize("delay", [False, True])
+def test_ar_with_per_sample_triggers_under_fm_bit_exact(port, reference, delay):
+    V, B, cap = 10, 200, 64
+    rng = np.random.default_rng(37)
+    p = W.voice_params(V, seed=37, delay_size=cap, ragged_delay=True)
+    att, _, rel = W.env_coeffs(p)
+    a, b = _pair(port, reference, V, osc="pulse", filt="lores", env="ar", delay=delay, delay_capacity=cap)
+    for k in (a, b):
+        _configure(k, "lores", p, delay=delay)
+        k.set("env_attack", att * 20.0); k.set("env_release", rel); k.set("env_holdtime", np.resize([1.0, 0.0, 3.0, 40.0], V))
+    for blk in range(3):
+        tv = (rng.random((B, V)) < 0.3).astype(np.uint8)
+        tv[:, 0] = 0; tv[:, 1] = 1; tv[::2, 2] = 1; tv[1::2, 2] = 0
+        f = _fm_outside_audio(V, B, blk)
+        oa, ma = a.process(B, freq_tv=f, trig_tv=tv, want_mix=True); ob, mb = b.process(B, freq_tv=f, trig_tv=tv, want_mix=True)
+        assert _same(oa, ob) and _same(ma, mb), blk
+        for s in ("env_amplitude", "env_output", "env_holdcount", "env_flags"):
+            assert _same(a.get(s), b.get(s)), (blk, s)
+
+
+def test_dl_from_position_with_fm_and_a_swept_cutoff_bit_exact(port, reference):
+    V, B, cap = 10, 150, 96
+    p = W.voice_params(V, seed=38, delay_size=cap, ragged_delay=True)
+    pos = np.array([0, 1, 5, 63, 95, 100, 200, 17, 40, 90], dtype=np.float64)     # >= size -> 0
+    a, b = _pair(port, reference, V, osc="phasorbetween", filt="svf", env=True, delay="position", delay_capacity=cap)
+    for k in (a, b):
+        _configure(k, "svf", p, env=True, delay=True)
+        k.set("delay_position", pos)
+    for blk in range(3):
+        f = _fm_outside_audio(V, B, blk); cu = cutoff_sweeps(V, B, blk)
+        on, off = W.gate(V, B, 4 * blk)
+        oa, ma = a.process(B, on, off, freq_tv=f, cutoff_tv=cu, want_mix=True); ob, mb = b.process(B, on, off, freq_tv=f, cutoff_tv=cu, want_mix=True)
+        assert _same(oa, ob) and _same(ma, mb), blk
+        assert same(a.get("delay_phase"), b.get("delay_phase"), equal_nan=False), blk
+    for v in range(V):
+        assert _same(a.ring(v, cap), b.ring(v, cap)), v
