@@ -471,6 +471,7 @@ int32_t mxb_mfcc_process(mxb_mfcc* m, const float* mags, int64_t n, double* coef
                          int32_t mem, void* stream);
 
 /* maxiIFFT::setup + process(mags, phases, SPECTRUM) per channel (src/libs/maxiFFT.cpp:141-192).
+ * fft_size: a power of two in [64, 2048]; hop_size: 1 .. fft_size (it need not divide fft_size). Anything else: MXB_ERR_INVALID.
  * mags/phases: frame f of channel c at (c*frames + f)*bins; out: planar float [channels][frames*hop]. */
 int32_t mxb_istft_create(mxb_ctx* ctx, int32_t channels, int32_t fft_size, int32_t hop_size, mxb_istft** st);
 int32_t mxb_istft_destroy(mxb_istft* st);

@@ -1006,6 +1006,7 @@ public:
     explicit maxiIFFT(int channels = 1, int device = 0) : C_(channels), device_(device) {}
     ~maxiIFFT() { if (h_) mxb_istft_destroy(h_); if (ctx_) mxb_ctx_destroy(ctx_); }
     maxiIFFT(const maxiIFFT&) = delete;
+    /* fftSize: a power of two from 64 to 2048, hopSize: 1 to fftSize -- every spectrum maxiFFT produces can be resynthesised */
     void setup(int fftSize = 1024, int hopSize = 512, int windowSize = 0) {
         using maxib200_detail::check;
         /* the reference windows with genWindow(3, windowSize ? windowSize : fftSize) (maxiFFT.cpp:141-152): another size is another window */
