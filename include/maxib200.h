@@ -269,6 +269,20 @@ int64_t mxb_bank_launch_count(const mxb_bank* bank);
 #define MXB_IN_F64 0                 /* input stream element types (mxb_patch_desc.input_types) */
 #define MXB_IN_U8 1                  /* unsigned bytes, read as (double)byte: triggers and gates (maxiEnv::trigger is an int) at 1 B / voice-sample */
 #define MXB_IN_BITS 2                /* one bit per voice-sample, read as 0.0 / 1.0: uint32 words [n_frames][(voices + 31) / 32], voice v = bit v % 32 of word v / 32 */
+#define MXB_IN_EVENTS 3              /* control events: per-voice values set at any frame and held (mxb_events); costs 16 B per event, not per voice-sample */
+/* An events stream: inputs[m] of mxb_patch_process points to one of these, in host memory; the three arrays live where `mem` says.
+ * Voice v's events are first[v] .. first[v+1]-1 (first[voices] is the count); a voice with first[v+1] <= first[v] has none.
+ * The stream reads the voice's HELD value. Its events apply in list order: event i takes effect at frame max(frame[i], the frame
+ * at which event i-1 took effect), before the stages of that sample read the stream. So for a sorted list the stream is the value
+ * of the last event with frame <= t (several on one frame: the last wins); a negative frame takes effect at frame 0; events at
+ * frames >= n_frames (and every later one of that voice) are dropped. The held value carries over to the next call; it starts at
+ * 0.0 (mxb_patch_get_held / set_held). A NULL descriptor or array, or with MXB_MEM_HOST a negative first[0] or a decreasing
+ * `first`, is MXB_ERR_INVALID. */
+typedef struct {
+    const int32_t* first;    /* [voices + 1] */
+    const int32_t* frame;    /* [first[voices]]: frame within this call of each event */
+    const double* value;     /* [first[voices]] */
+} mxb_events;
 /* oscillator kinds of MXB_OP_OSC beyond MXB_OSC_*: the table oscillators (tables: mxb_ctx_set_tables) */
 enum { MXB_OSC_SINEBUF = 9 /* maxiOsc::sinebuf src/maximilian.cpp:266-274 */, MXB_OSC_SINEBUF4 = 10 /* :237-264 */, MXB_OSC_SAWN = 11 /* :342-359 */ };
 /* filter kinds of MXB_OP_FILTER beyond MXB_FILT_LORES / HIRES */
@@ -339,7 +353,10 @@ int32_t mxb_patch_set_param(mxb_patch* patch, int32_t j, const double* values, i
 int32_t mxb_patch_set_state(mxb_patch* patch, int32_t stage, int32_t slot, const double* values, int32_t mem);
 int32_t mxb_patch_get_state(mxb_patch* patch, int32_t stage, int32_t slot, double* values, int32_t mem);
 int32_t mxb_patch_get_ring(mxb_patch* patch, int32_t stage, int32_t voice, double* dst, int32_t n, int32_t mem);
-/* inputs: n_inputs pointers to [n_frames][voices] of each stream's element type (MXB_IN_BITS: [n_frames][(voices + 31) / 32] words); out: [n_frames][voices] or NULL; mix: [n_frames][2] or NULL */
+/* the held values [voices] of events stream m (MXB_IN_EVENTS): to start a voice at a given value, or to checkpoint a patch. Any other stream is MXB_ERR_INVALID. */
+int32_t mxb_patch_get_held(mxb_patch* patch, int32_t m, double* values, int32_t mem);
+int32_t mxb_patch_set_held(mxb_patch* patch, int32_t m, const double* values, int32_t mem);
+/* inputs: n_inputs pointers to [n_frames][voices] of each stream's element type (MXB_IN_BITS: [n_frames][(voices + 31) / 32] words; MXB_IN_EVENTS: an mxb_events); out: [n_frames][voices] or NULL; mix: [n_frames][2] or NULL */
 int32_t mxb_patch_process(mxb_patch* patch, int32_t n_frames, const void* const* inputs, double* out, double* mix, int32_t mem, void* stream);
 int64_t mxb_patch_launch_count(const mxb_patch* patch);
 #define MXB_PATCH_INTERPRET 0

@@ -110,6 +110,45 @@ struct maxiStream {
 };
 
 class maxiVoices;
+/* Control events of the current block, for one value of every voice: the reference's play() writes members such as currentPitch or
+ * ADSR[voice].trigger on some samples, and the value holds until the next write. The control code calls set(frame, voice, value) during the
+ * block; render() hands the events over as an MXB_IN_EVENTS stream -- per voice, in call order -- and clears them. The stream reads each
+ * voice's held value: it starts at 0.0 and carries over from block to block (mxb_patch_get_held / set_held on patchHandle()). For a list
+ * in frame order that is the value of the last event at or before the sample; an event at a negative frame applies at frame 0, one at
+ * frame >= nFrames is dropped with every later one of that voice. It costs 16 bytes per event, where a maxiStream costs 8 per voice-sample.
+ * Usable wherever a maxiStream is, and as any stage argument (maxiArg).
+ * A one-sample trigger (the reference sets `trigger = 1` on a tick and back to 0 after that sample) is two events: set(t, v, 1) and
+ * set(t + 1, v, 0); when t is the block's last frame, the second belongs at frame 0 of the next block. */
+class maxiEvents {
+public:
+    explicit maxiEvents(maxiVoices& v);
+    void set(int frame, int voice, double value) {
+        if (voice < 0 || voice >= V_) throw maxiError(MXB_ERR_INVALID, "maxiEvents::set: voice " + std::to_string(voice) + " of " + std::to_string(V_));
+        ev_.push_back(Ev{voice, frame, value});
+    }
+private:
+    friend class maxiVoices;
+    struct Ev { int32_t voice, frame; double value; };
+    /* the events of this block as a CSR list by voice (a stable counting sort: each voice keeps its call order); then cleared */
+    const mxb_events* pack() {
+        first_.assign((size_t)V_ + 1, 0);
+        for (const Ev& e : ev_) first_[(size_t)e.voice + 1] += 1;
+        for (int v = 0; v < V_; ++v) first_[(size_t)v + 1] += first_[(size_t)v];
+        frame_.resize(ev_.size()); value_.resize(ev_.size());
+        std::vector<int32_t> at(first_.begin(), first_.end() - 1);
+        for (const Ev& e : ev_) { const size_t i = (size_t)at[(size_t)e.voice]++; frame_[i] = e.frame; value_[i] = e.value; }
+        ev_.clear();
+        desc_.first = first_.data(); desc_.frame = frame_.data(); desc_.value = value_.data();
+        return &desc_;
+    }
+    maxiVoices* v_;
+    int V_;
+    std::vector<Ev> ev_;
+    std::vector<int32_t> first_, frame_;
+    std::vector<double> value_;
+    mxb_events desc_{};
+};
+
 /* The signal flowing between the calls of a play(): a handle to a value of the recorded program (register, parameter or constant). */
 struct maxiSignal {
     maxiVoices* voices = nullptr;
@@ -188,18 +227,20 @@ public:
         return MXB_PARAM(nParams_++);
     }
     int32_t operand(const maxiSignal& x) { check(x, "operand"); return x.src; }
-    int32_t operand(const maxiStream& st) {
-        if ((size_t)nInputs_ >= inputPtr_.size()) inputPtr_.push_back(nullptr);
-        inputPtr_[(size_t)nInputs_] = st.values;
-        return MXB_INPUT(nInputs_++);
-    }
+    int32_t operand(const maxiStream& st) { return input(st.values, MXB_IN_F64, nullptr); }
     int32_t operand(const maxiGate& g) {          /* an interval gate: a trigger stream built at render time (or the bank's own gate) */
         gate_ = g;
-        if ((size_t)nInputs_ >= inputPtr_.size()) inputPtr_.push_back(nullptr);
         gateInput_ = nInputs_;
-        inputPtr_[(size_t)nInputs_] = nullptr;
-        return MXB_INPUT(nInputs_++);
+        return input(nullptr, MXB_IN_F64, nullptr);
     }
+    int32_t operand(const maxiEvents& ev) {       /* one events stream per maxiEvents object and block, however often it is read */
+        if (ev.v_ != this) throw maxiError(MXB_ERR_UNSUPPORTED, "maxiEvents: the events belong to another maxiVoices");
+        for (int k = 0; k < nInputs_; ++k) if (inputEv_[(size_t)k] == &ev) return MXB_INPUT(k);
+        return input(nullptr, MXB_IN_EVENTS, const_cast<maxiEvents*>(&ev));
+    }
+    /* a stream or events as a signal of play(), for the arithmetic between the calls (`currentPitch * 0.5`): no stage of its own */
+    maxiSignal signal(const maxiStream& st) { return maxiSignal{this, operand(st), 0}; }
+    maxiSignal signal(const maxiEvents& ev) { return maxiSignal{this, operand(ev), 0}; }
     maxiSignal emit(int32_t op, int32_t kind, std::initializer_list<int32_t> srcs, bool wantDst = true, int stageTag = 0) {
         mxb_stage g;
         g.op = op; g.kind = kind; g.reserved = 0; g.dst = MXB_NONE;
@@ -222,10 +263,15 @@ public:
 
 private:
     static bool blockConstant(int32_t s) { return s == MXB_NONE || (s >> 8) == 1 || (s >> 8) == 2; }   /* parameter or constant */
+    int32_t input(const double* values, int32_t type, maxiEvents* ev) {
+        if ((size_t)nInputs_ >= inputPtr_.size()) { inputPtr_.push_back(nullptr); inputType_.push_back(MXB_IN_F64); inputEv_.push_back(nullptr); }
+        inputPtr_[(size_t)nInputs_] = values; inputType_[(size_t)nInputs_] = type; inputEv_[(size_t)nInputs_] = ev;
+        return MXB_INPUT(nInputs_++);
+    }
     bool sameProgram() const {
         return built_.size() == prog_.size() && std::memcmp(built_.data(), prog_.data(), sizeof(mxb_stage) * prog_.size()) == 0 &&
                builtConsts_.size() == consts_.size() && std::memcmp(builtConsts_.data(), consts_.data(), sizeof(double) * consts_.size()) == 0 &&
-               builtShapes_ == egShapes_;
+               builtShapes_ == egShapes_ && std::vector<int32_t>(inputType_.begin(), inputType_.begin() + nInputs_) == builtTypes_;
     }
     /* the shape of one maxiEnvGen object (maxiEnvGen::setup, setLoop, setRetrigger) */
     struct EgShape {
@@ -303,12 +349,12 @@ private:
             std::memset(&d, 0, sizeof(d));
             d.voices = V_; d.n_stages = (int32_t)prog_.size(); d.n_params = nParams_; d.n_consts = (int32_t)consts_.size(); d.n_inputs = nInputs_;
             d.max_frames = maxFrames; d.delay_taps = delayCapacity_ > 0 ? delayCapacity_ : taps_;
-            d.stages = prog_.data(); d.consts = consts_.data();
+            d.stages = prog_.data(); d.consts = consts_.data(); d.input_types = inputType_.data();
             std::vector<mxb_envgen_shape> shapes;
             for (const EgShape& s : egShapes_) shapes.push_back({(int32_t)s.times.size(), s.loop, s.retrigger, s.levels.data(), s.times.data(), s.curves.data()});
             check(mxb_patch_create2(ctx_, &d, (int32_t)shapes.size(), shapes.data(), &patch_), "mxb_patch_create2");
         }
-        built_ = prog_; builtConsts_ = consts_; builtShapes_ = egShapes_;
+        built_ = prog_; builtConsts_ = consts_; builtShapes_ = egShapes_; builtTypes_.assign(inputType_.begin(), inputType_.begin() + nInputs_);
         for (size_t j = 0; j < paramDirty_.size(); ++j) paramDirty_[j] = true;
     }
 
@@ -366,6 +412,7 @@ private:
                     for (int t = (*gate_.on)[(size_t)v] < 0 ? 0 : (*gate_.on)[(size_t)v]; t < (*gate_.off)[(size_t)v] && t < nFrames; ++t) gateStream_[(size_t)t * (size_t)V_ + (size_t)v] = 1.0;
             inputPtr_[(size_t)gateInput_] = gateStream_.data();
         }
+        for (int k = 0; k < nInputs_; ++k) if (inputEv_[(size_t)k]) inputPtr_[(size_t)k] = inputEv_[(size_t)k]->pack();
         check(mxb_patch_process(patch_, nFrames, nInputs_ ? (const void* const*)inputPtr_.data() : nullptr, outSrc_ != MXB_NONE ? out : nullptr, wantMix_ ? mix : nullptr,
                                 MXB_MEM_HOST, nullptr), "mxb_patch_process");
     }
@@ -379,7 +426,9 @@ private:
     std::vector<double> consts_, builtConsts_;
     std::vector<std::vector<double>> paramVals_;
     std::vector<bool> paramDirty_;
-    std::vector<const double*> inputPtr_;
+    std::vector<const void*> inputPtr_;           /* per input stream: its data (an mxb_events for an events stream), type and maxiEvents */
+    std::vector<int32_t> inputType_, builtTypes_;
+    std::vector<maxiEvents*> inputEv_;
     std::vector<double> gateStream_;
     std::vector<std::pair<int, std::vector<double>>> pendingPhase_;      /* maxiOsc::phaseReset: (stage, per-voice phase), applied before the block */
     std::vector<const void*> egObjs_;                                     /* the maxiEnvGen objects that played in this block, by shape index */
@@ -392,6 +441,8 @@ private:
     maxiGate gate_;
     Chain chain_;
 };
+
+inline maxiEvents::maxiEvents(maxiVoices& v) : v_(&v), V_(v.size()) {}
 
 /* the arithmetic a play() does between the calls: recorded like everything else */
 namespace maxib200_detail {
@@ -418,9 +469,18 @@ public:
     maxiArg(int v) : par_((double)v) {}
     maxiArg(const std::vector<double>& v) : par_(v) {}
     maxiArg(const maxiParam& p) : par_(p) {}
-    int32_t op(maxiVoices* v) const { if (isSig_) { v->check(sig_, "argument"); return sig_.src; } return v->operand(par_); }
+    maxiArg(const maxiStream& s) : stream_(s.values), isStream_(true) {}
+    maxiArg(const maxiEvents& e) : ev_(&e) {}
+    int32_t op(maxiVoices* v) const {
+        if (isSig_) { v->check(sig_, "argument"); return sig_.src; }
+        if (isStream_) return v->operand(maxiStream(stream_));
+        if (ev_) return v->operand(*ev_);
+        return v->operand(par_);
+    }
 private:
     maxiSignal sig_; maxiParam par_; bool isSig_ = false;
+    const double* stream_ = nullptr; bool isStream_ = false;
+    const maxiEvents* ev_ = nullptr;
 };
 
 /* maxiOsc, src/maximilian.h:169-215 / src/maximilian.cpp:209-373 */
@@ -580,6 +640,7 @@ public:
 private:
     int32_t trig(const maxiSignal& s) { v_->check(s, "maxiEnvGen::play"); return s.src; }
     int32_t trig(const maxiStream& s) { return v_->operand(s); }
+    int32_t trig(const maxiEvents& e) { return v_->operand(e); }
     int32_t trig(const maxiParam& p) { return v_->operand(p); }
     maxiVoices* v_;
     maxiVoices::EgShape shape_;
@@ -623,7 +684,8 @@ private:
 class maxiChorus {
 public:
     maxiChorus(maxiVoices& v, int capacity) : v_(&v), capacity_(capacity) {}
-    maxiSignal chorus(maxiSignal input, const maxiArg& delay, const maxiArg& feedback, const maxiArg& speed, const maxiArg& depth, const maxiStream& noise) {
+    template <class Noise>      /* maxiStream or maxiEvents */
+    maxiSignal chorus(maxiSignal input, const maxiArg& delay, const maxiArg& feedback, const maxiArg& speed, const maxiArg& depth, const Noise& noise) {
         v_->check(input, "maxiChorus::chorus"); v_->delayCapacity_ = capacity_;
         return v_->emit(MXB_OP_CHORUS, 0, {input.src, delay.op(v_), feedback.op(v_), speed.op(v_), depth.op(v_), v_->operand(noise)});
     }

@@ -33,7 +33,7 @@ EXPORTS = [
     "mxb_octave_create", "mxb_octave_destroy", "mxb_octave_n_averages", "mxb_octave_config", "mxb_stft_process3",
     "mxb_ctx_set_tables", "mxb_patch_create", "mxb_patch_destroy", "mxb_patch_set_param", "mxb_patch_set_state", "mxb_patch_get_state",
     "mxb_patch_get_ring", "mxb_patch_process", "mxb_patch_launch_count", "mxb_patch_set_mode", "mxb_patch_get_mode", "mxb_patch_codegen",
-    "mxb_patch_create2",
+    "mxb_patch_create2", "mxb_patch_get_held", "mxb_patch_set_held",
     "mxb_octave_process", "mxb_bark_create", "mxb_bark_destroy", "mxb_bark_process",
 ]
 
@@ -136,6 +136,8 @@ def lib():
         "mxb_patch_get_mode": (i32, [vp]),
         "mxb_patch_codegen": (i32, [vp, vp, i64, vp, i32]),
         "mxb_patch_create2": (i32, [vp, vp, i32, vp, pp]),
+        "mxb_patch_get_held": (i32, [vp, i32, vp, i32]),
+        "mxb_patch_set_held": (i32, [vp, i32, vp, i32]),
         "mxb_octave_process": (i32, [vp, vp, i32, i32, vp, vp, i32, vp]),
         "mxb_bark_create": (i32, [vp, i32, i32, pp]),
         "mxb_bark_destroy": (i32, [vp]),
@@ -642,6 +644,11 @@ class PatchDesc(C.Structure):
                 ("input_types", C.POINTER(C.c_int32))]
 
 
+class Events(C.Structure):
+    """mxb_events: one call's events of an MXB_IN_EVENTS stream (CSR by voice)"""
+    _fields_ = [("first", C.c_void_p), ("frame", C.c_void_p), ("value", C.c_void_p)]
+
+
 class EnvgenShape(C.Structure):
     _fields_ = [("stages", C.c_int32), ("loop", C.c_int32), ("retrigger", C.c_int32),
                 ("levels", C.POINTER(C.c_double)), ("times", C.POINTER(C.c_double)), ("curves", C.POINTER(C.c_double))]
@@ -683,6 +690,19 @@ def pack_bits(x):
     return np.ascontiguousarray(np.packbits(pad, axis=1, bitorder="little")).view(np.uint32).reshape(n, W)
 
 
+def pack_events(lists):
+    """Per-voice lists of (frame, value) pairs -> the CSR triple of an events stream: first int32 [V + 1], frame int32 [n], value
+    float64 [n]. Each voice's events keep their list order (the order in which they apply)."""
+    first = np.zeros(len(lists) + 1, dtype=np.int32)
+    first[1:] = np.cumsum([len(x) for x in lists])
+    frame = np.array([f for x in lists for f, _ in x], dtype=np.int32)
+    value = np.array([v for x in lists for _, v in x], dtype=np.float64)
+    return first, frame, value
+
+
+IN_TYPE = {"u8": 1, "bits": 2, "events": 3}      # MXB_IN_*; doubles (MXB_IN_F64 = 0) otherwise
+
+
 def _patch_desc(defn, voices, max_frames, delay_taps):
     """mxb_patch_desc of a PatchDef; the second value keeps the ctypes arrays it points into alive."""
     st = (Stage * len(defn.stages))()
@@ -694,7 +714,7 @@ def _patch_desc(defn, voices, max_frames, delay_taps):
     # one shape travels in the descriptor (mxb_patch_create); several go to mxb_patch_create2 (Patch) and the descriptor's eg_* stay empty
     eg = defn.eg if defn.eg is not None and len(defn.shapes) == 1 else ([0.0], [], [], False, False)
     lv = (C.c_double * max(1, len(eg[0])))(*eg[0]); tm = (C.c_double * max(1, len(eg[1])))(*eg[1]); cv = (C.c_double * max(1, len(eg[2])))(*eg[2])
-    ty = (C.c_int32 * max(1, len(defn.inputs)))(*[{"u8": 1, "bits": 2}.get(defn.input_types.get(n), 0) for n in defn.inputs])
+    ty = (C.c_int32 * max(1, len(defn.inputs)))(*[IN_TYPE.get(defn.input_types.get(n), 0) for n in defn.inputs])
     d = PatchDesc(int(voices), len(defn.stages), len(defn.params), len(defn.consts), len(defn.inputs), int(max_frames), int(delay_taps),
                   len(eg[1]), int(eg[3]), int(eg[4]), st, consts, lv, tm, cv, ty)
     return d, (st, consts, lv, tm, cv, ty)
@@ -771,16 +791,37 @@ class Patch:
         check(lib().mxb_patch_get_ring(self.h, stage, v, _np_ptr(a), n, MEM_HOST), "mxb_patch_get_ring")
         return a
 
+    def get_held(self, name):
+        """the held values [V] of events stream `name`"""
+        a = np.empty(self.V, dtype=np.float64)
+        check(lib().mxb_patch_get_held(self.h, self.defn.inputs.index(name), _np_ptr(a), MEM_HOST), "mxb_patch_get_held")
+        return a
+
+    def set_held(self, name, values):
+        a = np.ascontiguousarray(np.broadcast_to(np.asarray(values, dtype=np.float64), (self.V,)))
+        check(lib().mxb_patch_set_held(self.h, self.defn.inputs.index(name), _np_ptr(a), MEM_HOST), "mxb_patch_set_held")
+
     @property
     def launches(self):
         return int(lib().mxb_patch_launch_count(self.h))
 
     def process(self, nframes, inputs=None, want_out=True, want_mix=False):
-        """inputs: dict name -> float64 [nframes][V]. Returns (out[nframes][V] | None, mix[nframes][2] | None)."""
+        """inputs: dict name -> float64 [nframes][V]; an events stream takes a CSR triple (first, frame, value) or per-voice lists of
+        (frame, value) pairs (pack_events). Returns (out[nframes][V] | None, mix[nframes][2] | None)."""
         inputs = inputs or {}
-        arrs = []
+        arrs, keep = [], []
         for n in self.defn.inputs:
             ty = self.defn.input_types.get(n)
+            if ty == "events":
+                x = inputs[n]
+                first, frame, value = x if isinstance(x, tuple) and len(x) == 3 and isinstance(x[0], np.ndarray) else pack_events(x)
+                first, frame = np.ascontiguousarray(first, dtype=np.int32), np.ascontiguousarray(frame, dtype=np.int32)
+                value = np.ascontiguousarray(value, dtype=np.float64)
+                assert first.shape == (self.V + 1,) and frame.shape == value.shape
+                d = Events(first.ctypes.data, frame.ctypes.data, value.ctypes.data)
+                keep += [first, frame, value]
+                arrs.append(d)
+                continue
             if ty == "bits":                 # [nframes][V] of 0 / 1 -> uint32 words [nframes][(V + 31) / 32], voice v = bit v % 32 of word v / 32
                 a = pack_bits(inputs[n])
                 assert a.shape == (nframes, (self.V + 31) // 32)
@@ -788,7 +829,7 @@ class Patch:
                 a = np.ascontiguousarray(inputs[n], dtype=np.uint8 if ty == "u8" else np.float64)
                 assert a.shape == (nframes, self.V)
             arrs.append(a)
-        ptrs = (C.c_void_p * max(1, len(arrs)))(*[a.ctypes.data for a in arrs])
+        ptrs = (C.c_void_p * max(1, len(arrs)))(*[C.addressof(a) if isinstance(a, Events) else a.ctypes.data for a in arrs])
         out = np.empty((nframes, self.V), dtype=np.float64) if want_out else None
         mix = np.empty((nframes, 2), dtype=np.float64) if want_mix else None
         check(lib().mxb_patch_process(self.h, nframes, ptrs, _np_ptr(out), _np_ptr(mix), MEM_HOST, None), "mxb_patch_process")

@@ -28,7 +28,10 @@ namespace {
 // MULTI_EG: the patch plays more than one maxiEnvGen shape. With one shape every ENVGEN stage plays shape 0, whose table and flags are then
 // read at fixed offsets of the argument block: a shape index read at run time makes ptxas spill in the stage loop, which cost the interpreter
 // about 2 % on the polysynth patch (H100 80GB HBM3, 700 W), a patch without any maxiEnvGen stage.
-template <bool MULTI_EG>
+// EVENTS: the patch has MXB_IN_EVENTS streams. Each keeps three words per voice in shared memory after the state -- its held value,
+// the cursor into this call's events and the frame of the event at the cursor -- advanced once per sample before the stage loop. A patch
+// without events streams runs the instantiation that has none of it: the same code, launch shape and shared-memory layout as before.
+template <bool MULTI_EG, bool EVENTS>
 __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a) {
     extern __shared__ double psm[];
     __shared__ mxb_stage s_stage[kMaxStages];
@@ -46,6 +49,12 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
     for (int i = 0; i < kMaxRegs; ++i) reg[i] = 0.0;
     for (int i = 0; i < a.n_params; ++i) par[i] = a.params[(size_t)i * V + vv];
     for (int i = 0; i < a.n_state; ++i) st[i] = a.state[(size_t)i * V + vv];
+    const Lane evl{psm + (size_t)(kMaxRegs + a.n_params + a.n_state) * kPatchThreads + tid, kPatchThreads};      // 3 words per events stream
+    if (EVENTS)
+        for (int e = 0; e < a.n_ev; ++e) {
+            evl[3 * e] = a.held[(size_t)e * V + vv];
+            ev_start(a.ev[e], vv, live, evl[3 * e + 1], evl[3 * e + 2]);
+        }
     __syncthreads();
     const int gwarp = (int)(((long long)blockIdx.x * blockDim.x + tid) >> 5);
     const double sr = a.sr;
@@ -53,6 +62,8 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
     for (int t = 0; t < a.n_frames; ++t) {
         double ml = 0.0, mr = 0.0;
         for (int i = 0; i < kMaxRegs; ++i) reg[i] = 0.0;          // registers read 0 until a stage of this sample writes them
+        if (EVENTS)
+            for (int e = 0; e < a.n_ev; ++e) ev_advance(a.ev[e], vv, t, evl[3 * e], evl[3 * e + 1], evl[3 * e + 2]);
         auto fetch = [&](const int src) -> double {
             if (src < 0) return 0.0;
             const int k = src & 0xff;
@@ -60,7 +71,9 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
                 case 0: return reg[k];
                 case 1: return par[k];
                 case 2: return s_const[k];
-                default: return live ? patch_input(a, k, (size_t)t, vv, V) : 0.0;
+                default:
+                    if (EVENTS && a.in_kind[k] == MXB_IN_EVENTS) return evl[3 * a.ev_of[k]];
+                    return live ? patch_input(a, k, (size_t)t, vv, V) : 0.0;
             }
         };
         for (int si = 0; si < a.n_stages; ++si) {
@@ -192,6 +205,7 @@ __global__ void __launch_bounds__(kPatchThreads) patch_kernel(const PatchArgs a)
         if (a.partials) mix_warp_store(ml, mr, lane, a.partials, (size_t)t, (size_t)a.W, (size_t)gwarp);      // the second kernel adds the warps in order
     }
     if (live) for (int i = 0; i < a.n_state; ++i) a.state[(size_t)i * V + (size_t)v] = st[i];
+    if (EVENTS && live) for (int e = 0; e < a.n_ev; ++e) a.held[(size_t)e * V + (size_t)v] = evl[3 * e];
 }
 
 // MXB_PATCH_MODE=interpret | fused overrides the default (fused) for patches created afterwards: an A/B and debugging hook
@@ -222,7 +236,7 @@ int validate_stages(const mxb_patch_desc* d, const int n_shapes, const char* who
                 MXB_ERR_INVALID, "%s: n_params %d n_consts %d n_inputs %d", who, d->n_params, d->n_consts, d->n_inputs);
     MXB_REQUIRE(d->n_consts == 0 || d->consts, MXB_ERR_INVALID, "%s: consts is NULL", who);
     for (int i = 0; d->input_types && i < d->n_inputs; ++i)
-        MXB_REQUIRE(d->input_types[i] >= MXB_IN_F64 && d->input_types[i] <= MXB_IN_BITS, MXB_ERR_INVALID, "%s: input_types[%d] = %d", who, i, d->input_types[i]);
+        MXB_REQUIRE(d->input_types[i] >= MXB_IN_F64 && d->input_types[i] <= MXB_IN_EVENTS, MXB_ERR_INVALID, "%s: input_types[%d] = %d", who, i, d->input_types[i]);
     for (int i = 0; i < d->n_stages; ++i) {
         const mxb_stage& g = d->stages[i];
         MXB_REQUIRE(g.op >= MXB_OP_OSC && g.op <= MXB_OP_CHORUS, MXB_ERR_INVALID, "%s: stage %d: unknown op %d", who, i, g.op);
@@ -283,8 +297,11 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
         n_state += patch_state_slots(g.op);
     }
     if (tables) MXB_REQUIRE(ctx->d_sine.get(), MXB_ERR_STATE, "%s: sinebuf / sinebuf4 / sawn need the reference's tables: call mxb_ctx_set_tables first", who);
-    const size_t per_thread = (size_t)(kMaxRegs + d->n_params + n_state);
-    MXB_REQUIRE(per_thread * 8 * kPatchThreads <= 200 * 1024, MXB_ERR_UNSUPPORTED, "%s: %zu doubles of registers, parameters and state per voice do not fit shared memory", who, per_thread);
+    int n_ev = 0;
+    for (int i = 0; d->input_types && i < d->n_inputs; ++i) n_ev += d->input_types[i] == MXB_IN_EVENTS;
+    const size_t per_thread = (size_t)(kMaxRegs + d->n_params + n_state + 3 * n_ev);
+    MXB_REQUIRE(per_thread * 8 * kPatchThreads <= 200 * 1024, MXB_ERR_UNSUPPORTED,
+                "%s: %zu doubles of registers, parameters, state and events streams (3 each) per voice do not fit shared memory", who, per_thread);
     DeviceGuard g(ctx->device);
     std::unique_ptr<mxb_patch> p(new (std::nothrow) mxb_patch());
     MXB_REQUIRE(p, MXB_ERR_ALLOC, "%s: out of host memory", who);
@@ -293,7 +310,12 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
     p->stages.assign(d->stages, d->stages + d->n_stages);
     if (d->n_consts) p->consts.assign(d->consts, d->consts + d->n_consts);
     p->mode = patch_default_mode(); p->fused = nullptr; p->ex = nullptr;
-    for (int i = 0; i < d->n_inputs; ++i) p->in_type[i] = d->input_types ? d->input_types[i] : MXB_IN_F64;
+    p->n_ev = 0;
+    for (int i = 0; i < d->n_inputs; ++i) {
+        p->in_type[i] = d->input_types ? d->input_types[i] : MXB_IN_F64;
+        p->ev_of[i] = (unsigned char)p->n_ev;
+        p->n_ev += p->in_type[i] == MXB_IN_EVENTS;
+    }
     int sb = 0, ri = 0;
     for (int i = 0; i < d->n_stages; ++i) {
         p->state_base.push_back(sb); sb += patch_state_slots(p->stages[i].op);
@@ -315,6 +337,7 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
     if (rc == MXB_OK) rc = p->state.alloc((size_t)(n_state ? n_state : 1) * V);
     if (rc == MXB_OK && n_rings) rc = p->rings.alloc((size_t)n_rings * (size_t)p->taps * V);
     if (rc == MXB_OK) rc = p->mix_dev.alloc((size_t)p->max_frames * 2);
+    if (rc == MXB_OK && p->n_ev) rc = p->held.alloc((size_t)p->n_ev * V);          // held values start at 0.0
     if (rc != MXB_OK) return rc;
     cudaError_t e = cudaMemcpy(p->d_stages.get(), p->stages.data(), sizeof(mxb_stage) * d->n_stages, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(p->d_state_base.get(), p->state_base.data(), sizeof(int) * d->n_stages, cudaMemcpyHostToDevice);
@@ -328,6 +351,37 @@ int32_t create_patch(mxb_ctx* ctx, const mxb_patch_desc* d, const int32_t n_shap
             }
     if (e != cudaSuccess) { set_error("%s: %s", who, cudaGetErrorString(e)); return MXB_ERR_CUDA; }
     *out = p.release();
+    return MXB_OK;
+}
+
+// The structural checks of an events descriptor (mxb_events): before any copy or kernel, so that a refused call changes nothing.
+// Device-memory arrays are not looked at: whatever they hold, the kernels read voice v's events only inside [first[v], first[v+1]).
+int check_events(const mxb_patch* p, const int m, const mxb_events* e, const bool host) {
+    MXB_REQUIRE(e->first && e->frame && e->value, MXB_ERR_INVALID, "mxb_patch_process: events stream %d: first / frame / value is NULL", m);
+    if (host) {
+        MXB_REQUIRE(e->first[0] >= 0, MXB_ERR_INVALID, "mxb_patch_process: events stream %d: first[0] = %d", m, e->first[0]);
+        for (int v = 0; v < p->V; ++v)
+            MXB_REQUIRE(e->first[v + 1] >= e->first[v], MXB_ERR_INVALID, "mxb_patch_process: events stream %d: first[%d] = %d < first[%d] = %d", m, v + 1,
+                        e->first[v + 1], v, e->first[v]);
+    }
+    return MXB_OK;
+}
+
+// the device view of events stream m for this call: host arrays through the patch's staging buffers (first[voices] events)
+int stage_events(mxb_patch* p, const int m, const mxb_events* e, const bool host, cudaStream_t s, EvStream* out) {
+    const int k = p->ev_of[m];
+    const size_t n = host ? (size_t)e->first[p->V] : 0;
+    int rc = stage_in(host, e->first, (size_t)p->V + 1, p->ev_first[k], s, &out->first);
+    if (rc == MXB_OK) rc = stage_in(host, e->frame, n, p->ev_frame[k], s, &out->frame);
+    if (rc == MXB_OK) rc = stage_in(host, e->value, n, p->ev_value[k], s, &out->value);
+    return rc;
+}
+
+// events stream m's held values ([voices] doubles)
+int32_t patch_held_ptr(mxb_patch* p, const int32_t m, double** ptr, const char* who) {
+    MXB_REQUIRE(p, MXB_ERR_INVALID, "%s: NULL patch", who);
+    MXB_REQUIRE(m >= 0 && m < p->n_inputs && p->in_type[m] == MXB_IN_EVENTS, MXB_ERR_INVALID, "%s: input stream %d is not an events stream", who, m);
+    *ptr = p->held.get() + (size_t)p->ev_of[m] * (size_t)p->V;
     return MXB_OK;
 }
 
@@ -420,6 +474,26 @@ int32_t mxb_patch_get_ring(mxb_patch* p, int32_t stage, int32_t voice, double* d
     return MXB_OK;
 }
 
+int32_t mxb_patch_get_held(mxb_patch* p, int32_t m, double* values, int32_t mem) {
+    double* src = nullptr;
+    const int rc = patch_held_ptr(p, m, &src, "mxb_patch_get_held");
+    if (rc != MXB_OK) return rc;
+    MXB_REQUIRE(values && (mem == MXB_MEM_HOST || mem == MXB_MEM_DEVICE), MXB_ERR_INVALID, "mxb_patch_get_held: bad argument");
+    DeviceGuard g(p->ctx->device);
+    MXB_CUDA(cudaMemcpy(values, src, sizeof(double) * (size_t)p->V, mem == MXB_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice));
+    return MXB_OK;
+}
+
+int32_t mxb_patch_set_held(mxb_patch* p, int32_t m, const double* values, int32_t mem) {
+    double* dst = nullptr;
+    const int rc = patch_held_ptr(p, m, &dst, "mxb_patch_set_held");
+    if (rc != MXB_OK) return rc;
+    MXB_REQUIRE(values && (mem == MXB_MEM_HOST || mem == MXB_MEM_DEVICE), MXB_ERR_INVALID, "mxb_patch_set_held: bad argument");
+    DeviceGuard g(p->ctx->device);
+    MXB_CUDA(cudaMemcpy(dst, values, sizeof(double) * (size_t)p->V, mem == MXB_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice));
+    return MXB_OK;
+}
+
 int64_t mxb_patch_launch_count(const mxb_patch* p) { return p ? p->launches : 0; }
 
 int32_t mxb_patch_set_mode(mxb_patch* p, int32_t mode) {
@@ -458,7 +532,13 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
     MXB_REQUIRE(n_frames >= 0 && n_frames <= p->max_frames, MXB_ERR_INVALID, "mxb_patch_process: n_frames %d (max_frames %d)", n_frames, p->max_frames);
     MXB_REQUIRE(mem == MXB_MEM_HOST || mem == MXB_MEM_DEVICE, MXB_ERR_INVALID, "mxb_patch_process: mem %d", mem);
     MXB_REQUIRE(p->n_inputs == 0 || inputs, MXB_ERR_INVALID, "mxb_patch_process: the patch reads %d input streams, inputs is NULL", p->n_inputs);
-    for (int i = 0; i < p->n_inputs; ++i) MXB_REQUIRE(inputs[i], MXB_ERR_INVALID, "mxb_patch_process: input stream %d is NULL", i);
+    for (int i = 0; i < p->n_inputs; ++i) {
+        MXB_REQUIRE(inputs[i], MXB_ERR_INVALID, "mxb_patch_process: input stream %d is NULL", i);
+        if (p->in_type[i] == MXB_IN_EVENTS) {
+            const int rc = check_events(p, i, (const mxb_events*)inputs[i], mem == MXB_MEM_HOST);
+            if (rc != MXB_OK) return rc;
+        }
+    }
     if (mix) {     // before any kernel runs: a refused call leaves every stage's state untouched
         const int rc = mix_bus_admit(p->ex, n_frames, "mxb_patch_process");
         if (rc != MXB_OK) return rc;
@@ -472,6 +552,12 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
     const bool host = mem == MXB_MEM_HOST;
     for (int i = 0; i < p->n_inputs; ++i) {
         a.in_kind[i] = (unsigned char)p->in_type[i];
+        if (p->in_type[i] == MXB_IN_EVENTS) {
+            const int rc = stage_events(p, i, (const mxb_events*)inputs[i], host, s, &a.ev[p->ev_of[i]]);
+            if (rc != MXB_OK) return rc;
+            a.ev_of[i] = p->ev_of[i];
+            continue;
+        }
         const unsigned char* d_in;
         const int rc = stage_in(host, (const unsigned char*)inputs[i], patch_input_bytes(p->in_type[i], (size_t)n_frames, V), p->in_stage[i], s, &d_in);
         if (rc != MXB_OK) return rc;
@@ -492,14 +578,16 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
     a.sine = sine; a.transition = sine ? sine + 514 : nullptr; a.sine_before = p->ctx->sine_before;
     memcpy(a.eg_n, p->eg_n, sizeof(a.eg_n)); memcpy(a.eg_loop, p->eg_loop, sizeof(a.eg_loop)); memcpy(a.eg_retrigger, p->eg_retrigger, sizeof(a.eg_retrigger));
     memcpy(a.eg, p->eg, sizeof(a.eg));
+    a.n_ev = p->n_ev; a.held = p->held.get();
     if (p->mode == MXB_PATCH_FUSED) {
         // the kernel generated for this stage list (patch_fuse.cu): compiled on first use, then launched like any other
         rc = patch_fused_load(p);
         if (rc == MXB_OK) rc = patch_fused_launch(p, a, grid, s);
         if (rc != MXB_OK) return rc;
     } else {
-        const size_t smem = sizeof(double) * (size_t)(kMaxRegs + p->n_params + p->n_state) * kPatchThreads;
-        void (*kernel)(const PatchArgs) = p->n_shapes > 1 ? patch_kernel<true> : patch_kernel<false>;
+        const size_t smem = sizeof(double) * (size_t)(kMaxRegs + p->n_params + p->n_state + 3 * p->n_ev) * kPatchThreads;
+        void (*kernel)(const PatchArgs) = p->n_ev ? (p->n_shapes > 1 ? patch_kernel<true, true> : patch_kernel<false, true>)
+                                                  : (p->n_shapes > 1 ? patch_kernel<true, false> : patch_kernel<false, false>);
         MXB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kernel<<<grid, kPatchThreads, smem, s>>>(a);
         MXB_CUDA(cudaGetLastError());

@@ -18,6 +18,9 @@ constexpr int kMaxEgShapes = 4;          // maxiEnvGen shapes of one patch (9.En
 
 struct EgStage { double startlevel, endlevel, gradient, curve; long long length; int hold; int pad; };
 
+// one call's events of an MXB_IN_EVENTS stream, on the device (mxb_events)
+struct EvStream { const int* first; const int* frame; const double* value; };
+
 struct PatchArgs {
     int V, n_frames, n_stages, n_params, n_state, W, taps;
     double sr;
@@ -37,6 +40,10 @@ struct PatchArgs {
     double sine_before;              // what sinebuf4 reads at sineBuffer[-1] on its wrap sample (out of bounds in the reference)
     int eg_n[kMaxEgShapes], eg_loop[kMaxEgShapes], eg_retrigger[kMaxEgShapes];      // shape k: an ENVGEN stage of kind k plays it
     EgStage eg[kMaxEgShapes][kMaxEg];
+    int n_ev;                        // events streams (MXB_IN_EVENTS), numbered in input order
+    unsigned char ev_of[kMaxInputs]; // input stream k -> its events stream number (events streams only)
+    EvStream ev[kMaxInputs];         // events stream e of this call
+    double* held;                    // [n_ev][V]: each events stream's held value, carried from call to call
 };
 static_assert(sizeof(PatchArgs) <= 4096, "PatchArgs must fit the 4 KB kernel parameter block");
 
@@ -312,6 +319,30 @@ __host__ __device__ inline size_t patch_input_bytes(const int kind, const size_t
     return kind == MXB_IN_BITS ? n_frames * ((V + 31) >> 5) * 4 : n_frames * V * (kind == MXB_IN_U8 ? 1 : 8);
 }
 
+// An events stream (MXB_IN_EVENTS) of voice v, shared by both kernels. The caller keeps the held value, the cursor into the voice's
+// events and the frame of the event at the cursor (kEvNever: none left), so that a sample with nothing due costs one compare. T: the
+// interpreter keeps cursor and frame as doubles in shared memory, a generated kernel as ints in registers.
+constexpr int kEvNever = 0x7fffffff;
+template <class T> __device__ __forceinline__ void ev_start(const EvStream& e, const size_t v, const bool live, T& cur, T& next) {
+    cur = 0; next = (T)kEvNever;
+    if (!live) return;
+    const int c = e.first[v], end = e.first[v + 1];
+    cur = (T)c;
+    if (c < end) next = (T)e.frame[c];
+}
+// before the stages of frame t read the stream: apply, in list order, every event due by t. Event i takes effect at max(its frame, the
+// frame event i-1 took effect at), so the reads stay inside [first[v], first[v+1]) whatever order the list is in.
+template <class T> __device__ __forceinline__ void ev_advance(const EvStream& e, const size_t v, const int t, double& held, T& cur, T& next) {
+    if (next > (T)t) return;
+    const int end = e.first[v + 1];
+    do {
+        const int c = (int)cur;
+        held = e.value[c];
+        cur = (T)(c + 1);
+        next = c + 1 < end ? (T)e.frame[c + 1] : (T)kEvNever;
+    } while (next <= (T)t);
+}
+
 }  // namespace mxb
 
 #ifndef __CUDACC_RTC__
@@ -328,6 +359,11 @@ struct mxb_patch {
     mxb::DevBuf<double> params, state, rings;
     mxb::DevBuf<unsigned char> in_stage[mxb::kMaxInputs];      // staging for MXB_MEM_HOST input streams (bytes)
     int in_type[mxb::kMaxInputs];
+    int n_ev;                                                  // MXB_IN_EVENTS streams; ev_of[k]: the number of input k among them
+    unsigned char ev_of[mxb::kMaxInputs];
+    mxb::DevBuf<double> held;                                  // [n_ev][V]
+    mxb::DevBuf<int> ev_first[mxb::kMaxInputs], ev_frame[mxb::kMaxInputs];     // staging for MXB_MEM_HOST events, by events stream
+    mxb::DevBuf<double> ev_value[mxb::kMaxInputs];
     mxb::DevBuf<double> out_stage, partials, mix_dev;
     int n_shapes;          // maxiEnvGen shapes; ENVGEN stage kinds index them
     int eg_n[mxb::kMaxEgShapes], eg_loop[mxb::kMaxEgShapes], eg_retrigger[mxb::kMaxEgShapes];

@@ -31,7 +31,7 @@ class PatchDef:
         self.consts = []
         self.params = []          # names, index = parameter slot
         self.inputs = []          # names, index = input stream
-        self.input_types = {}     # name -> "u8" | "bits" for byte / packed-bit streams (triggers, gates); doubles otherwise
+        self.input_types = {}     # name -> "u8" | "bits" for byte / packed-bit streams (triggers, gates), "events" for control events; doubles otherwise
         self.eg = None            # maxiEnvGen shape 0: (levels, times, curves, loop, retrigger)
 
     def K(self, value):
@@ -54,11 +54,11 @@ class PatchDef:
 
     def IN(self, name, dtype="f64"):
         """per-sample input stream operand; dtype "u8": the caller passes unsigned bytes, "bits": one bit per voice-sample packed into
-        uint32 words (both read as doubles by the stages)"""
+        uint32 words (both read as doubles by the stages), "events": per-voice values set at any frame and held (MXB_IN_EVENTS)"""
         if name not in self.inputs:
             self.inputs.append(name)
             assert len(self.inputs) <= 8
-            if dtype in ("u8", "bits"):
+            if dtype in ("u8", "bits", "events"):
                 self.input_types[name] = dtype
         return 0x300 + self.inputs.index(name)
 

@@ -124,6 +124,44 @@ def polysynth_patch(trigger_dtype="f64"):
     return d
 
 
+def polysynth_pitch_patch(pitch_dtype="events", trigger_dtype="events"):
+    """polysynth_patch with the voice's pitch as a stream too (f1 = 55 * pitch, f2 = 110 * pitch, the cutoff from pitch + LFO): the shape
+    of a host-driven synth that plays a new note on any sample. "events" (MXB_IN_EVENTS) costs per change, "f64" per voice-sample."""
+    from .patchdef import PatchDef, R
+    d = PatchDef()
+    one = d.K(1.0)
+    pitch = d.IN("pitch", pitch_dtype)
+    d.stage("env_adsr", one, d.IN("trigger", trigger_dtype), d.P("attack"), d.P("decay"), d.P("sustain"), d.P("release"), d.K(1.0), dst=R(0))
+    d.stage("osc", d.K(0.2), kind="sinebuf", dst=R(1))
+    d.stage("mul", d.K(55.0), pitch, dst=R(8))
+    d.stage("osc", R(8), d.K(0.6), kind="pulse", dst=R(2))
+    d.stage("mul", d.K(110.0), pitch, dst=R(9))
+    d.stage("add", R(9), R(1), dst=R(3))
+    d.stage("osc", R(3), d.K(0.2), kind="pulse", dst=R(3))
+    d.stage("add", R(2), R(3), dst=R(4))
+    d.stage("mul", R(4), d.K(0.5), dst=R(4))
+    d.stage("add", pitch, R(1), dst=R(5))
+    d.stage("mul", R(5), d.K(1000.0), dst=R(5))
+    d.stage("add", d.K(250.0), R(5), dst=R(5))
+    d.stage("filter", R(4), R(5), d.K(10.0), kind="lores", dst=R(6))
+    d.stage("mul", R(6), R(0), dst=R(7))
+    d.stage("div", R(7), d.K(6.0), dst=R(7))
+    d.stage("out", R(7))
+    d.stage("mix_stereo", R(7), d.P("pan"))
+    return d
+
+
+def note_events(voices, block, block_index, seed=SEED):
+    """about one note per voice per block: a new pitch (1 .. 6) at a random frame t < block - 1, and a one-sample trigger (1 at t, 0 at
+    t + 1). CSR triples (first, frame, value) of the pitch and of the trigger events."""
+    rng = np.random.default_rng(seed + 505 + block_index)
+    t = rng.integers(0, block - 1, voices).astype(np.int32)
+    pitch = 1.0 + rng.integers(0, 6, voices).astype(np.float64)
+    pe = (np.arange(voices + 1, dtype=np.int32), t, pitch)
+    te = ((2 * np.arange(voices + 1)).astype(np.int32), np.stack([t, t + 1], axis=1).reshape(-1), np.tile([1.0, 0.0], voices))
+    return pe, te
+
+
 def polysynth_params(voices, seed=SEED):
     p = voice_params(voices, seed=seed)
     att, dec, rel = env_coeffs(p)
