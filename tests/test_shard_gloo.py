@@ -125,3 +125,22 @@ def test_two_rank_sharded_voice_patch_matches_the_whole_patch(port):
             assert np.array_equal(outs[blk], out[:, lo:hi])
             np.testing.assert_allclose(buses[blk], mix, rtol=1e-12, atol=1e-12)
     assert np.array_equal(res[0][4], res[1][4])
+
+
+def test_events_stream_shards_are_the_voices_of_the_whole_stream():
+    """tests/exchange_ranks.slice_events (each rank's part of a whole-bank events stream) against a per-voice loop over the whole stream"""
+    import events_checks as EV
+    from exchange_ranks import slice_events
+    from maximilian_b200 import capi
+    rng = np.random.default_rng(4)
+    V, n = 37, 64
+    whole = capi.pack_events(EV.random_events(rng, V, n))
+    first, frame, value = whole
+    for world in (1, 2, 3, 4, 8, 37):
+        for rank in range(world):
+            lo, hi = shard.shard_range(V, rank, world)
+            lists = [[(int(frame[i]), float(value[i])) for i in range(first[v], first[v + 1])] for v in range(lo, hi)]
+            want = capi.pack_events(lists)
+            got = slice_events(whole, lo, hi)
+            for g, w, what in zip(got, want, ("first", "frame", "value")):
+                assert g.dtype == w.dtype and np.array_equal(g, w), (world, rank, what)
