@@ -517,6 +517,7 @@ int32_t mxo_get_tables(double* sine514, double* transition1001, double* sine_bef
 }
 
 typedef struct { double startlevel, endlevel, currentlevel, gradient, curve; size_t length, counter; int hold; } eg_stage_t;
+typedef struct { eg_stage_t seg[MXO_MAX_EG_SEGMENTS]; int n, loop, retrigger; } eg_shape_t;    /* one maxiEnvGen after setup() */
 
 typedef struct {
     mxo_patch_desc d;
@@ -528,7 +529,7 @@ typedef struct {
     double* state;    /* [n_state][V] */
     double* rings;    /* [n_rings][V][taps] */
     double reg[16];
-    eg_stage_t eg[16];
+    eg_shape_t eg[MXO_MAX_EG_SHAPES];
 } patch_t;
 
 static int p_state_slots(const mxo_stage* g) {
@@ -556,9 +557,10 @@ void mxo_noise_fill(uint32_t seed, int64_t n, double* out) {
 }
 
 void* mxo_patch_create(const mxo_patch_desc* d) {
-    if (!d || d->voices <= 0 || d->n_stages <= 0 || d->n_stages > 64 || !d->stages) return NULL;
+    if (!d || d->voices <= 0 || d->n_stages <= 0 || d->n_stages > 64 || !d->stages || !mxo_patch_shapes_ok(d)) return NULL;
     patch_t* p = (patch_t*)calloc(1, sizeof(patch_t));
     p->d = *d;
+    p->d.shapes = NULL;                                    /* copied into p->eg below */
     p->stages = (mxo_stage*)malloc(sizeof(mxo_stage) * (size_t)d->n_stages);
     memcpy(p->stages, d->stages, sizeof(mxo_stage) * (size_t)d->n_stages);
     p->consts = (double*)calloc(64, sizeof(double));
@@ -578,14 +580,17 @@ void* mxo_patch_create(const mxo_patch_desc* d) {
     for (int i = 0; i < d->n_stages; ++i)
         if (p->stages[i].op == MXO_OP_ENVGEN)
             for (int k = 6; k < 12; ++k) for (size_t v = 0; v < V; ++v) p->state[(size_t)(p->sbase[i] + k) * V + v] = 1.0;
-    /* maxiEnvGen::setup / setupSegmentTime, src/maximilian.h:2371-2402, 2524-2538 */
-    {
+    /* maxiEnvGen::setup / setupSegmentTime, src/maximilian.h:2371-2402, 2524-2538, once per shape: each is its own object */
+    for (int k = 0; k < d->n_shapes; ++k) {
+        const mxo_envgen_shape* sh = &d->shapes[k];
+        eg_shape_t* e = &p->eg[k];
+        e->n = sh->stages; e->loop = sh->loop; e->retrigger = sh->retrigger;
         double accumulatedTime = 0;
         const double sr = (double)(size_t)d->sample_rate;
-        for (int i = 0; i < d->eg_stages && i < 16; ++i) {
-            eg_stage_t* s = &p->eg[i];
-            s->startlevel = d->eg_levels[i]; s->endlevel = d->eg_levels[i + 1];
-            const double stageTime = d->eg_times[i];
+        for (int i = 0; i < sh->stages; ++i) {
+            eg_stage_t* s = &e->seg[i];
+            s->startlevel = sh->levels[i]; s->endlevel = sh->levels[i + 1];
+            const double stageTime = sh->times[i];
             if (stageTime == MXO_ENVGEN_HOLD) { s->length = 0; s->hold = 1; s->gradient = 0; }
             else {
                 double len = ((stageTime / 1000.0) * sr) + accumulatedTime;
@@ -594,7 +599,7 @@ void* mxo_patch_create(const mxo_patch_desc* d) {
                 s->gradient = 1.0 / s->length;
                 s->hold = 0;
             }
-            s->curve = d->eg_curves[i]; s->counter = 0; s->currentlevel = 0;
+            s->curve = sh->curves[i]; s->counter = 0; s->currentlevel = 0;
         }
     }
     return p;
@@ -730,10 +735,10 @@ static double p_on_zx(double* previousValue, double* firstTrigger, double input)
 
 /* maxiEnvGen::play, src/maximilian.h:2276-2357; the per-stage counter / currentlevel of the reference are zero for every
  * stage but the current one, so one pair per voice carries them */
-static double p_envgen(const patch_t* p, double* st, size_t V, double trigger) {
+static double p_envgen(const eg_shape_t* e, double* st, size_t V, double trigger) {
     double envval = st[0]; size_t phase = (size_t)st[V]; int state = (int)st[2 * V]; int nxc = st[3 * V] != 0.0;
     size_t counter = (size_t)st[4 * V]; double currentlevel = st[5 * V];
-    const size_t nst = (size_t)p->d.eg_stages;
+    const size_t nst = (size_t)e->n;
     int run = 1;
 #define P_RESET() do { counter = 0; currentlevel = 0; phase = 0; state = 1; } while (0)
     if (state == 0) {
@@ -741,7 +746,7 @@ static double p_envgen(const patch_t* p, double* st, size_t V, double trigger) {
         else run = 0;
     }
     if (run && state == 1) {
-        const eg_stage_t* cs = &p->eg[phase < nst ? phase : 0];
+        const eg_stage_t* cs = &e->seg[phase < nst ? phase : 0];
         if (p_on_zx(&st[8 * V], &st[9 * V], -trigger)) nxc = 1;
         if (cs->hold) state = 2;
         else {
@@ -752,16 +757,16 @@ static double p_envgen(const patch_t* p, double* st, size_t V, double trigger) {
             counter++;
             if (counter == cs->length) { counter = 0; currentlevel = 0; phase++; }
             else currentlevel += cs->gradient;
-            if (p->d.eg_retrigger) { if (p_on_zx(&st[10 * V], &st[11 * V], trigger)) { nxc = 0; P_RESET(); } }
+            if (e->retrigger) { if (p_on_zx(&st[10 * V], &st[11 * V], trigger)) { nxc = 0; P_RESET(); } }
             run = 0;
         }
     }
     if (run && state == 2) {
         if (p_on_zx(&st[8 * V], &st[9 * V], -trigger)) nxc = 1;
         if (nxc) { state = 1; phase++; }
-        if (p->d.eg_retrigger) { if (p_on_zx(&st[10 * V], &st[11 * V], trigger)) { nxc = 0; P_RESET(); } }
+        if (e->retrigger) { if (p_on_zx(&st[10 * V], &st[11 * V], trigger)) { nxc = 0; P_RESET(); } }
     }
-    if (phase == nst) { P_RESET(); if (!p->d.eg_loop) state = 0; }
+    if (phase == nst) { P_RESET(); if (!e->loop) state = 0; }
 #undef P_RESET
     st[0] = envval; st[V] = (double)phase; st[2 * V] = (double)state; st[3 * V] = nxc ? 1.0 : 0.0; st[4 * V] = (double)counter; st[5 * V] = currentlevel;
     return envval;
@@ -809,7 +814,7 @@ int32_t mxo_patch_process(void* h, int32_t nframes, const double* const* inputs,
                     case MXO_OP_ENV_AR:
                         y = p_env_ar(st, V, FETCH(g->src[0]), (int)FETCH(g->src[1]), FETCH(g->src[2]), FETCH(g->src[3]), (long)FETCH(g->src[4]));
                         break;
-                    case MXO_OP_ENVGEN: y = p_envgen(p, st, V, FETCH(g->src[0])); break;
+                    case MXO_OP_ENVGEN: y = p_envgen(&p->eg[g->kind], st, V, FETCH(g->src[0])); break;
                     case MXO_OP_FILTER: {
                         const double input = FETCH(g->src[0]);
                         if (g->kind == MXO_FILT_LORES || g->kind == MXO_FILT_HIRES) {

@@ -155,14 +155,34 @@ enum { MXO_OP_OSC = 1, MXO_OP_ENV_ADSR, MXO_OP_ENV_AR, MXO_OP_ENVGEN, MXO_OP_FIL
        MXO_OP_DELAY, MXO_OP_FLANGER, MXO_OP_ADD, MXO_OP_SUB, MXO_OP_MUL, MXO_OP_DIV, MXO_OP_MIX_STEREO, MXO_OP_OUT,
        MXO_OP_CHORUS /* maxiChorus::chorus, src/maximilian.h:1200-1212: src5 = the value maxiOsc::noise() returns this sample */ };
 typedef struct { int32_t op, kind, dst, reserved; int32_t src[8]; } mxo_stage;      /* operands: 0..15 register, 0x100+j parameter, 0x200+k constant, 0x300+m input, -1 none */
+/* one maxiEnvGen shape, the arguments of maxiEnvGen::setup (src/maximilian.h:2371-2402), as mxb_envgen_shape: levels[stages + 1],
+ * times[stages], curves[stages]. A shape of no segments is a maxiEnvGen whose setup() was never called (levels[0] only). */
+typedef struct {
+    int32_t stages, loop, retrigger;
+    const double *levels, *times, *curves;
+} mxo_envgen_shape;
+enum { MXO_MAX_EG_SHAPES = 4, MXO_MAX_EG_SEGMENTS = 16 };                                  /* the library's limits */
+/* An ENVGEN stage plays shapes[kind]; mxo_patch_create returns NULL for a kind outside [0, n_shapes) or a shape list past the limits.
+ * Both libraries copy what they need at create time: the arrays may be freed afterwards. */
 typedef struct {
     int32_t voices, n_stages, n_params, n_consts, n_inputs, sample_rate;
     int32_t delay_taps;
-    int32_t eg_stages, eg_loop, eg_retrigger;
+    int32_t n_shapes;
     const mxo_stage* stages;
     const double* consts;
-    const double *eg_levels, *eg_times, *eg_curves;
+    const mxo_envgen_shape* shapes;
 } mxo_patch_desc;
+/* the shape checks of mxo_patch_create, shared by both libraries */
+static inline int mxo_patch_shapes_ok(const mxo_patch_desc* d) {
+    if (d->n_shapes < 0 || d->n_shapes > MXO_MAX_EG_SHAPES || (d->n_shapes > 0 && !d->shapes)) return 0;
+    for (int k = 0; k < d->n_shapes; ++k) {
+        const mxo_envgen_shape* s = &d->shapes[k];
+        if (s->stages < 0 || s->stages > MXO_MAX_EG_SEGMENTS || !s->levels || (s->stages > 0 && (!s->times || !s->curves))) return 0;
+    }
+    for (int i = 0; i < d->n_stages; ++i)
+        if (d->stages[i].op == MXO_OP_ENVGEN && (d->stages[i].kind < 0 || d->stages[i].kind >= d->n_shapes)) return 0;
+    return 1;
+}
 /* sineBuffer[514] / transition[1001] of the reference (src/maximilian.cpp:63, 67-200) and the double before sineBuffer[0] that
  * sinebuf4 reads on its wrap sample. The compiled reference returns its own; the port is handed them (mxo_set_tables). */
 int32_t mxo_set_tables(const double* sine514, const double* transition1001, double sine_before);

@@ -355,11 +355,19 @@ class MxoStage(C.Structure):
     _fields_ = [("op", C.c_int32), ("kind", C.c_int32), ("dst", C.c_int32), ("reserved", C.c_int32), ("src", C.c_int32 * 8)]
 
 
+class MxoEnvgenShape(C.Structure):
+    _fields_ = [("stages", C.c_int32), ("loop", C.c_int32), ("retrigger", C.c_int32),
+                ("levels", C.POINTER(C.c_double)), ("times", C.POINTER(C.c_double)), ("curves", C.POINTER(C.c_double))]
+
+
 class MxoPatchDesc(C.Structure):
     _fields_ = [("voices", C.c_int32), ("n_stages", C.c_int32), ("n_params", C.c_int32), ("n_consts", C.c_int32), ("n_inputs", C.c_int32),
-                ("sample_rate", C.c_int32), ("delay_taps", C.c_int32), ("eg_stages", C.c_int32), ("eg_loop", C.c_int32), ("eg_retrigger", C.c_int32),
-                ("stages", C.POINTER(MxoStage)), ("consts", C.POINTER(C.c_double)),
-                ("eg_levels", C.POINTER(C.c_double)), ("eg_times", C.POINTER(C.c_double)), ("eg_curves", C.POINTER(C.c_double))]
+                ("sample_rate", C.c_int32), ("delay_taps", C.c_int32), ("n_shapes", C.c_int32),
+                ("stages", C.POINTER(MxoStage)), ("consts", C.POINTER(C.c_double)), ("shapes", C.POINTER(MxoEnvgenShape))]
+
+
+def _doubles(x):
+    return (C.c_double * max(1, len(x)))(*x)
 
 
 def _patch_sigs(lib):
@@ -437,12 +445,16 @@ class Patch:
             st[i].op, st[i].kind, st[i].dst, st[i].reserved = op, k, dst, 0
             for j in range(8):
                 st[i].src[j] = src[j]
-        consts = (C.c_double * max(1, len(defn.consts)))(*defn.consts)
-        eg = defn.eg or ([0.0], [], [], False, False)
-        lv = (C.c_double * max(1, len(eg[0])))(*eg[0]); tm = (C.c_double * max(1, len(eg[1])))(*eg[1]); cv = (C.c_double * max(1, len(eg[2])))(*eg[2])
+        consts = _doubles(defn.consts)
+        shapes = (MxoEnvgenShape * max(1, len(defn.shapes)))()
+        keep = [st, consts, shapes]
+        for i, (lv, tm, cv, loop, retrig) in enumerate(defn.shapes):
+            arrs = _doubles(lv), _doubles(tm), _doubles(cv)
+            shapes[i] = MxoEnvgenShape(len(tm), int(loop), int(retrig), *arrs)
+            keep += arrs
         d = MxoPatchDesc(self.V, len(defn.stages), len(defn.params), len(defn.consts), len(defn.inputs), sample_rate, int(delay_taps),
-                         len(eg[1]), int(eg[3]), int(eg[4]), st, consts, lv, tm, cv)
-        self._keep = (st, consts, lv, tm, cv)
+                         len(defn.shapes), st, consts, shapes)
+        self._keep = keep
         self.h = self.lib.mxo_patch_create(C.byref(d))
         if not self.h:
             raise RuntimeError("mxo_patch_create failed")

@@ -492,10 +492,11 @@ int32_t mxo_get_tables(double* sine514, double* transition1001, double* sine_bef
 }
 
 void* mxo_patch_create(const mxo_patch_desc* d) {
-    if (!d || d->voices <= 0 || d->n_stages <= 0 || d->n_stages > 64 || !d->stages) return nullptr;
+    if (!d || d->voices <= 0 || d->n_stages <= 0 || d->n_stages > 64 || !d->stages || !mxo_patch_shapes_ok(d)) return nullptr;
     maxiSettings::setup((size_t)d->sample_rate, 2, 1024);
     RefPatch* p = new RefPatch();
     p->d = *d;
+    p->d.shapes = nullptr;                                               /* each stage's maxiEnvGen objects are set up below */
     p->stages.assign(d->stages, d->stages + d->n_stages);
     p->consts.assign(64, 0.0);
     for (int i = 0; i < d->n_consts; ++i) p->consts[i] = d->consts[i];
@@ -511,11 +512,11 @@ void* mxo_patch_create(const mxo_patch_desc* d) {
         if (g.op == MXO_OP_DELAY) { dl = (maxiDelayline**)calloc((size_t)V, sizeof(void*)); for (int v = 0; v < V; ++v) dl[v] = zeroed_new<maxiDelayline>(); }
         if (g.op == MXO_OP_FLANGER) { fl = (maxiFlanger**)calloc((size_t)V, sizeof(void*)); for (int v = 0; v < V; ++v) fl[v] = zeroed_new<maxiFlanger>(); }
         if (g.op == MXO_OP_ENVGEN) {
+            const mxo_envgen_shape& s = d->shapes[g.kind];
             eg = new maxiEnvGen[V];
-            std::vector<double> levels(d->eg_levels, d->eg_levels + d->eg_stages + 1), times(d->eg_times, d->eg_times + d->eg_stages),
-                curves(d->eg_curves, d->eg_curves + d->eg_stages);
+            std::vector<double> levels(s.levels, s.levels + s.stages + 1), times(s.times, s.times + s.stages), curves(s.curves, s.curves + s.stages);
             std::streambuf* old = std::cout.rdbuf(nullptr);              /* setup() prints every segment */
-            for (int v = 0; v < V; ++v) eg[v].setup(levels, times, curves, d->eg_loop != 0, d->eg_retrigger != 0);
+            for (int v = 0; v < V; ++v) eg[v].setup(levels, times, curves, s.loop != 0, s.retrigger != 0);
             std::cout.rdbuf(old);
         }
         p->delays.push_back(dl); p->flangers.push_back(fl); p->choruses.push_back(ch); p->envgens.push_back(eg);

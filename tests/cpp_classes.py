@@ -343,7 +343,7 @@ def patch_cases():
         return d, dict(trig=0, tf=1), {}
     c.append(_patch("envgen_triggers", "src/maximilian.h:2276 maxiEnvGen::play(trigger), :2371 setup(levels, times, curves, looping, allowRetrigger), "
                     "setupAR / setupASR / setupADSR, setLoop, setRetrigger", [BLOCKS((1.0, 0.0), (0.0, 1.0), (1.0,)), U(100.0, 900.0)],
-                    envgen, False, shapes=True))
+                    envgen, False))
 
     def arith():
         d = PatchDef()

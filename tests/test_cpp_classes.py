@@ -11,7 +11,6 @@ import numpy as np
 import pytest
 
 import cpp_classes as CC
-import envgen_oracle as EO
 import golden_checks as G
 import patch_checks as PK
 from maximilian_b200.patchdef import OP, STATE_SLOTS
@@ -226,10 +225,7 @@ def _patch_oracle(port, c):
     if getattr(c, "fix", None):
         c.fix(d, lib)
     PK.set_tables(port, library=False)
-    if getattr(c, "shapes", False):
-        o = EO.ShapesPatch(port, d, V, sample_rate=c.sr, delay_taps=c.cap, kind="port")
-    else:
-        o = port.Patch(d, V, sample_rate=c.sr, delay_taps=c.cap, kind="port")
+    o = port.Patch(d, V, sample_rate=c.sr, delay_taps=c.cap, kind="port")
     outs = []
     for blk in range(NB):
         P, _, _, S = c.data(V, B, blk)

@@ -1,6 +1,6 @@
 """9.Envelopes2 through the C++ layer (tests/cpp/patch_envelopes.cpp): three maxiEnvGen objects, each with its own setup(), in one play().
 It compiles against include/maximilian_b200.hpp (CPU check) and, on the GPU, its output equals the C oracle running the same graph with
-the three shapes (tests/envgen_cases.py, tests/envgen_oracle.py), in both ways a patch runs."""
+the three shapes (tests/envgen_cases.py), in both ways a patch runs."""
 import os
 import subprocess
 
@@ -8,7 +8,6 @@ import numpy as np
 import pytest
 
 import envgen_cases as EC
-import envgen_oracle as EO
 from test_cpp_dropin import ROOT, compile_patch
 
 SRC = os.path.join(ROOT, "tests", "cpp", "patch_envelopes.cpp")
@@ -37,7 +36,7 @@ def test_envelopes_port_matches_oracle(port, tmp_path, bindir, mode):
     r = subprocess.run([exe, str(tmp_path / "out.bin"), str(NB), str(B)], capture_output=True, text=True, env=env)
     assert r.returncode == 0, r.stderr
     out = np.fromfile(tmp_path / "out.bin", dtype=np.float64).reshape(NB * B, V)
-    o = EO.ShapesPatch(port, EC.envelopes2(), V, sample_rate=44100, kind="port")
+    o = port.Patch(EC.envelopes2(), V, sample_rate=44100, kind="port")
     oo, _ = o.process(NB * B)
     peak = np.abs(oo).max()
     assert peak > 1e-2
@@ -46,5 +45,5 @@ def test_envelopes_port_matches_oracle(port, tmp_path, bindir, mode):
     # the silent failure this guards against: every maxiEnvGen playing the shape of the last setup() (myEnv3) sounds far from it
     d = EC.envelopes2()
     d.stages = [(op, 2 if op == 4 else k, dst, src) for op, k, dst, src in d.stages]
-    ow, _ = EO.ShapesPatch(port, d, V, sample_rate=44100, kind="port").process(NB * B)
+    ow, _ = port.Patch(d, V, sample_rate=44100, kind="port").process(NB * B)
     assert np.abs(ow - out).max() > 0.1 * peak

@@ -9,7 +9,6 @@ import pytest
 from maximilian_b200 import capi
 from maximilian_b200.patchdef import PatchDef, R, ENVGEN_HOLD
 import envgen_cases as EC
-import envgen_oracle as EO
 
 MODES = ["fused", "interpret"]
 BLOCKS = [1, 17, 1024]
@@ -52,7 +51,7 @@ def test_envgen_shapes_match_oracle(port, case, mode):
     V = 333                                                # a partial last warp
     ins = inputs(V, sum(BLOCKS), 21)
     g = capi.Patch(d, V, max_frames=1024, mode=mode)
-    o = EO.ShapesPatch(port, d, V, kind="port")
+    o = port.Patch(d, V, kind="port")
     for k, v in params(V, 4).items():
         g.set(k, v); o.set(k, v)
     for n, x in _blocks(ins):
