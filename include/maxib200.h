@@ -19,7 +19,9 @@
  *     copies out and returns when the results are in host memory) or MXB_MEM_DEVICE (asynchronous on
  *     `stream`, a cudaStream_t passed as void*; NULL = the legacy default stream).
  *   - one handle is driven from one thread/stream at a time (like the reference objects, which are
- *     owned by the audio thread); different handles are independent.
+ *     owned by the audio thread); different handles are independent, also when they are called from
+ *     different host threads at the same time. Host-memory calls on the NULL stream of one context
+ *     still run one after another on the device.
  *   - sample values are fp64 for the oscillator/filter/envelope/delay/mix path (the reference's
  *     `double`), fp32 for the FFT path (the reference's `float`), fp64 for MFCCs.
  */

@@ -24,6 +24,11 @@ namespace mxb {
 
 void set_error(const char* fmt, ...);
 
+// Makes the current device's dynamic shared-memory limit of `kern` at least `bytes` before a launch that asks for `bytes`. The limit
+// belongs to the kernel, shared by every handle and host thread, so it is only ever raised: a launch on another thread that needs
+// less cannot lower it between this thread's check and its launch. Every launch with dynamic shared memory goes through here.
+int smem_limit_at_least(const void* kern, size_t bytes, const char* what);
+
 #define MXB_CUDA(expr)                                                                         \
     do {                                                                                       \
         cudaError_t _e = (expr);                                                               \

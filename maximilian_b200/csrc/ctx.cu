@@ -1,5 +1,8 @@
-// Context, error reporting and the envelope-setter helpers of libmaxib200.so.
+// Context, error reporting, kernels' shared-memory limits and the envelope-setter helpers of libmaxib200.so.
 #include <math.h>
+
+#include <map>
+#include <mutex>
 
 #include "common.cuh"
 
@@ -10,6 +13,23 @@ void set_error(const char* fmt, ...) {
     va_start(ap, fmt);
     vsnprintf(g_err, sizeof(g_err), fmt, ap);
     va_end(ap);
+}
+
+int smem_limit_at_least(const void* kern, size_t bytes, const char* what) {
+    static std::mutex mu;
+    static std::map<std::pair<int, const void*>, size_t> limit;       // (device, kernel) -> the limit this process set
+    int dev = 0;
+    MXB_CUDA(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lk(mu);                                   // held across the set: two raises cannot land out of order
+    size_t& cur = limit[{dev, kern}];
+    if (bytes <= cur) return MXB_OK;
+    const cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) {
+        set_error("%s: dynamic shared memory limit %zu B: %s", what, bytes, cudaGetErrorString(e));
+        return MXB_ERR_CUDA;
+    }
+    cur = bytes;
+    return MXB_OK;
 }
 }  // namespace mxb
 

@@ -397,10 +397,10 @@ inline int launch_delay_one(const BankArgs& a, const DelayArgs& d, cudaStream_t 
     constexpr size_t smem = sizeof(double) * (threads / 32) * (kDlStages * kStageDoubles + (MIX ? kMixDoubles : 0));
     const int grid = (a.V + threads - 1) / threads;
     auto kern = delay_bank_kernel<OSC, FILT, ENV, OUTMODE, MIX, MODK>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { set_error("delay_bank_kernel smem attribute (%zu B): %s", smem, cudaGetErrorString(e)); return MXB_ERR_CUDA; }
+    const int rc = smem_limit_at_least((const void*)kern, smem, "delay_bank_kernel");
+    if (rc != MXB_OK) return rc;
     kern<<<grid, threads, smem, s>>>(a, d);
-    e = cudaGetLastError();
+    const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("delay_bank_kernel launch: %s", cudaGetErrorString(e)); return MXB_ERR_CUDA; }
     return MXB_OK;
 }

@@ -588,7 +588,8 @@ int32_t mxb_patch_process(mxb_patch* p, int32_t n_frames, const void* const* inp
         const size_t smem = sizeof(double) * (size_t)(kMaxRegs + p->n_params + p->n_state + 3 * p->n_ev) * kPatchThreads;
         void (*kernel)(const PatchArgs) = p->n_ev ? (p->n_shapes > 1 ? patch_kernel<true, true> : patch_kernel<false, true>)
                                                   : (p->n_shapes > 1 ? patch_kernel<true, false> : patch_kernel<false, false>);
-        MXB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        rc = smem_limit_at_least((const void*)kernel, smem, "patch_kernel");
+        if (rc != MXB_OK) return rc;
         kernel<<<grid, kPatchThreads, smem, s>>>(a);
         MXB_CUDA(cudaGetLastError());
     }

@@ -109,3 +109,22 @@ CASES = [
     ("delay_size", _delay_size, lambda rng, k: rng.integers(1, 64, k).astype(np.float64), 64),
     ("pan", _pan, lambda rng, k: rng.uniform(-0.2, 1.2, k), 0),
 ]
+
+
+def budget_patch(flanger, ty):
+    """doubles per voice: 16 registers + 32 parameters + 3 for each of 8 events streams + the stages' state: 61 oscillators (122), an
+    AR envelope (4) and either one more oscillator (2: 200 in all) or a flanger (3: 201)"""
+    d = PatchDef()
+    for j in range(32):
+        d.P(f"p{j}")
+    for j in range(8):
+        d.IN(f"e{j}", ty)
+    for s in range(61):
+        d.stage("osc", d.P(f"p{s % 32}") if s else d.IN("e0", ty), kind="sinewave", dst=R(s % 8))
+    d.stage("env_ar", R(0), d.IN("e1", ty), d.K(0.01), d.K(0.999), d.K(1.0), dst=R(8))
+    if flanger:
+        d.stage("flanger", R(8), d.K(4.0), d.K(0.5), d.K(1.0), d.K(0.5), dst=R(9))
+    else:
+        d.stage("osc", d.IN("e7", ty), kind="saw", dst=R(9))
+    d.stage("out", R(9))
+    return d

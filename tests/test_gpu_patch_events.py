@@ -147,34 +147,15 @@ def test_malformed_descriptors_are_refused_and_change_nothing():
     assert np.array_equal(p.get_held("x"), np.full(V, 440.0))
 
 
-def _budget_patch(flanger, ty):
-    """doubles per voice: 16 registers + 32 parameters + 3 for each of 8 events streams + the stages' state: 61 oscillators (122), an
-    AR envelope (4) and either one more oscillator (2: 200 in all) or a flanger (3: 201)"""
-    d = PatchDef()
-    for j in range(32):
-        d.P(f"p{j}")
-    for j in range(8):
-        d.IN(f"e{j}", ty)
-    for s in range(61):
-        d.stage("osc", d.P(f"p{s % 32}") if s else d.IN("e0", ty), kind="sinewave", dst=R(s % 8))
-    d.stage("env_ar", R(0), d.IN("e1", ty), d.K(0.01), d.K(0.999), d.K(1.0), dst=R(8))
-    if flanger:
-        d.stage("flanger", R(8), d.K(4.0), d.K(0.5), d.K(1.0), d.K(0.5), dst=R(9))
-    else:
-        d.stage("osc", d.IN("e7", ty), kind="saw", dst=R(9))
-    d.stage("out", R(9))
-    return d
-
-
 def test_interpreter_budget_counts_events_streams():
     """200 doubles per voice fit and 201 are refused, with the 3 words of each events stream counted; the 201-double stage list over
     dense streams (no events words) fits. The 200-double patch runs on the interpreter bit for bit as the generated kernel does."""
     V, n = 200, 64
     rng = np.random.default_rng(3)
     with pytest.raises(capi.MxbError, match="-> -4"):
-        capi.Patch(_budget_patch(True, "events"), V, max_frames=n, delay_taps=8, mode="interpret")
-    capi.Patch(_budget_patch(True, "f64"), V, max_frames=n, delay_taps=8, mode="interpret")
-    d200 = _budget_patch(False, "events")
+        capi.Patch(EV.budget_patch(True, "events"), V, max_frames=n, delay_taps=8, mode="interpret")
+    capi.Patch(EV.budget_patch(True, "f64"), V, max_frames=n, delay_taps=8, mode="interpret")
+    d200 = EV.budget_patch(False, "events")
     a = capi.Patch(d200, V, max_frames=n, mode="interpret"); b = capi.Patch(d200, V, max_frames=n, mode="fused")
     for p in (a, b):
         for j in range(32):
