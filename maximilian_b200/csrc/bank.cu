@@ -5,6 +5,7 @@
 
 #include <new>
 #include <thread>
+#include <type_traits>
 
 #include "bank_kernels.cuh"
 #include "delay_kernels.cuh"
@@ -131,6 +132,23 @@ int upload_fill(double* dst, size_t n, double value) {
     std::vector<double> h(n, value);
     MXB_CUDA(cudaMemcpy(dst, h.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
     return MXB_OK;
+}
+
+// Calls launch(std::integral_constant<int, filt_t>()) for a filter family FILT_T_*: the one place that maps a family to the
+// instantiations built for it (launch_bank_filt, launch_delay_filt; build.py builds one object per family)
+template <class L>
+int with_filt(const int filt_t, L&& launch) {
+    switch (filt_t) {
+        case FILT_T_NONE:   return launch(std::integral_constant<int, FILT_T_NONE>());
+        case FILT_T_LORES:  return launch(std::integral_constant<int, FILT_T_LORES>());
+        case FILT_T_HIRES:  return launch(std::integral_constant<int, FILT_T_HIRES>());
+        case FILT_T_SVF:    return launch(std::integral_constant<int, FILT_T_SVF>());
+        case FILT_T_SVF_LP: return launch(std::integral_constant<int, FILT_T_SVF_LP>());
+        case FILT_T_BIQUAD: return launch(std::integral_constant<int, FILT_T_BIQUAD>());
+        default: break;
+    }
+    set_error("bank: filter family %d", filt_t);
+    return MXB_ERR_UNSUPPORTED;
 }
 
 }  // namespace
@@ -546,8 +564,16 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
     else if (b->desc.osc_kind == MXB_OSC_SAW) osc_t = OSC_T_SAW;
     const int env = b->desc.env_kind != MXB_ENV_NONE ? 1 : 0;
     a.env_ar = b->desc.env_kind == MXB_ENV_AR ? 1 : 0;
-    const bool svf_lp = fk == MXB_FILT_SVF && b->desc.svf_mix[0] == 1.0 && b->desc.svf_mix[1] == 0.0 &&
-                        b->desc.svf_mix[2] == 0.0 && b->desc.svf_mix[3] == 0.0;
+    // the filter family of the instantiations: the SVF with mix (1, 0, 0, 0) runs the low-pass-only one
+    int filt_t = FILT_T_NONE;
+    switch (fk) {
+        case MXB_FILT_LORES:  filt_t = FILT_T_LORES; break;
+        case MXB_FILT_HIRES:  filt_t = FILT_T_HIRES; break;
+        case MXB_FILT_SVF:    filt_t = b->desc.svf_mix[0] == 1.0 && b->desc.svf_mix[1] == 0.0 && b->desc.svf_mix[2] == 0.0 &&
+                                       b->desc.svf_mix[3] == 0.0 ? FILT_T_SVF_LP : FILT_T_SVF; break;
+        case MXB_FILT_BIQUAD: filt_t = FILT_T_BIQUAD; break;
+        default: break;
+    }
 
     if (b->desc.delay_taps > 0) {
         DelayArgs da;
@@ -555,21 +581,21 @@ int32_t mxb_bank_process_mod(mxb_bank* b, int32_t n_frames, const mxb_modulation
         da.ring = b->ring.get(); da.taps = b->desc.delay_taps;
         da.from_position = b->desc.delay_mode == MXB_DELAY_FROM_POSITION ? 1 : 0; da.position = b->dl_pos.get();
         da.size_tv = d_ds;
-        rc = launch_delay_bank(a, da, fk, svf_lp, env, out != nullptr, mix != nullptr, s);
-        if (rc != MXB_OK) return rc;
+        const int saw = a.osc_kind == MXB_OSC_SAW;
+        const int outmode = !out ? 0 : (a.out_f32 ? 2 : 1);      // DL_OUT_NONE / F64 / F32
+        const bool modk = a.freq_tv || a.cutoff_tv;               // per-sample frequency / cutoff: the modulated instantiations
+        rc = with_filt(filt_t, [&](auto f) {
+            constexpr int F = decltype(f)::value;
+            return modk ? launch_delay_filt<F, true>(a, da, saw, env, outmode, mix != nullptr, s)
+                        : launch_delay_filt<F, false>(a, da, saw, env, outmode, mix != nullptr, s);
+        });
     } else {
-        bank_launch_fn fn = launch_bank_none;
-        switch (fk) {
-            case MXB_FILT_LORES: fn = launch_bank_lores; break;
-            case MXB_FILT_HIRES: fn = launch_bank_hires; break;
-            case MXB_FILT_SVF: fn = svf_lp ? launch_bank_svf_lp : launch_bank_svf; break;
-            case MXB_FILT_BIQUAD: fn = launch_bank_biquad; break;
-            default: break;
-        }
         const size_t smem = mix ? sizeof(double) * (kBankBlock / 32) * 2 * kMixTT * 33 : 0;
-        rc = fn(a, osc_t, env, out != nullptr, mix != nullptr, grid, smem, s);
-        if (rc != MXB_OK) return rc;
+        rc = with_filt(filt_t, [&](auto f) {
+            return launch_bank_filt<decltype(f)::value>(a, osc_t, env, out != nullptr, mix != nullptr, grid, smem, s);
+        });
     }
+    if (rc != MXB_OK) return rc;
     b->launches += 1;
     if (mix) {
         rc = mix_bus_reduce(b->ex, b->partials.get(), W, n_frames, d_mix, s);

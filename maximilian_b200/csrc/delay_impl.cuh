@@ -1,5 +1,5 @@
-// K2: oscillator -> [envelope] -> [filter] -> maxiDelayline::dl -> out / stereo mix.   (kernel template; the
-// instantiations live in delay_k_*.cu, one translation unit per filter family, the dispatcher in delay.cu)
+// K2: oscillator -> [envelope] -> [filter] -> maxiDelayline::dl -> out / stereo mix.   (kernel template; delay_k.cu instantiates it,
+// once per filter family and MODK)
 //
 // maxiDelayline::dl (src/maximilian.cpp:420-429) reads ring[phase] and writes it back every sample:
 // 8 B read + 8 B write of ring traffic per voice-sample on top of the 8 B output -- the one genuinely
@@ -101,7 +101,7 @@ struct DlVoice {
 // MODW: the block carries a per-sample oscillator frequency (a.freq_tv) and / or filter cutoff (a.cutoff_tv): the reference takes both
 // by argument on every call (FM: maximilian_examples/5.FM1/main.cpp:29), so the increment / the filter design are redone each sample,
 // in the order the patch evaluates them (oscillator, envelope, design, filter). Its own instantiation of the window body;
-// modulated blocks run their own instantiation of the KERNEL (MODK; delay_km_*.cu), so the block-constant kernels are compiled exactly
+// modulated blocks run their own instantiation of the KERNEL (MODK; objects delay_km_*.o), so the block-constant kernels are compiled exactly
 // as before (with both bodies in one kernel the headline instantiation was slower).
 template <int OSC, int FILT, int ENV, bool ALLFAST, int OUTMODE, bool MIX, bool ESTEADY, bool MODW = false>
 __device__ __forceinline__ void dl_stage(DlVoice& s, double* row, const int tn, const int t0, const BankArgs& a, const DelayArgs& d,
@@ -232,31 +232,12 @@ __global__ void __launch_bounds__(DelayShape<MIX>::kThreads, DelayShape<MIX>::kM
     DlVoice s;
     s.live = v < a.V;
     const long long vv = s.live ? v : 0;
-    s.phase = a.phase[vv]; s.oout = a.osc_out[vv];
-    const bool pb = OSC == OSC_T_GENERIC && a.osc_kind == MXB_OSC_PHASORBETWEEN;      // duty / pend carry startphase / endphase
-    s.duty = (OSC == OSC_T_GENERIC) ? (pb ? a.pstart[vv] : a.duty[vv]) : 0.0;
-    s.pend = pb ? a.pend[vv] : 0.0;
-    s.inc = pb ? ((s.pend - s.duty) / (a.sr / (a.freq[vv]))) : (1. / (a.sr / (a.freq[vv])));
-    if (FILT != FILT_T_NONE) {
-        s.fr.s0 = a.f0[vv]; s.fr.s1 = a.f1[vv]; s.fr.s2 = (FILT == FILT_T_SVF || FILT == FILT_T_SVF_LP) ? a.f2[vv] : 0.0;
-        s.fr.c0 = a.cf[0][vv]; s.fr.c1 = a.cf[1][vv];
-        if (FILT != FILT_T_LORES && FILT != FILT_T_HIRES) { s.fr.c2 = a.cf[2][vv]; s.fr.c3 = a.cf[3][vv]; s.fr.c4 = a.cf[4][vv]; }
-    }
+    osc_load<OSC>(a, vv, s.phase, s.oout, s.inc, s.duty, s.pend);
+    filt_load<FILT>(a, vv, s.fr);
     s.res = (MODK && a.cutoff_tv) ? a.res[vv] : 0.0;
-    if (ENV) {
-        s.er.amp = a.env_amp[vv]; s.er.output = a.env_output[vv];
-        s.er.att = a.env_att[vv]; s.er.dec = a.env_dec[vv]; s.er.sus = a.env_sus[vv]; s.er.rel = a.env_rel[vv];
-        s.er.holdcount = (int)a.env_holdcount[vv]; s.er.holdtime = (int)a.env_hold[vv]; env_unpack(s.er, a.env_flags[vv]);
-        s.er.on = a.trig_on ? a.trig_on[vv] : 0; s.er.off = a.trig_off ? a.trig_off[vv] : 0;
-    }
+    env_load<ENV>(a, vv, s.er);
     s.gl = s.gr = 0.0;
-    if (MIX) {
-        double x = a.pan[vv];
-        if (x > 1) x = 1;
-        if (x < 0) x = 0;
-        s.gl = s.live ? sqrt(1.0 - x) : 0.0;
-        s.gr = s.live ? sqrt(x) : 0.0;
-    }
+    if (MIX) stereo_gains(a.pan[vv], s.live, s.gl, s.gr);
     s.ph = d.phase[vv];
     s.size = d.size[vv];
     s.fb = d.feedback[vv];
@@ -380,13 +361,7 @@ __global__ void __launch_bounds__(DelayShape<MIX>::kThreads, DelayShape<MIX>::kM
     }
 
     if (s.live) {
-        a.phase[v] = s.phase;
-        a.osc_out[v] = s.oout;
-        if (FILT != FILT_T_NONE) {
-            a.f0[v] = s.fr.s0; a.f1[v] = s.fr.s1;
-            if (FILT == FILT_T_SVF || FILT == FILT_T_SVF_LP) a.f2[v] = s.fr.s2;
-        }
-        if (ENV) { a.env_amp[v] = s.er.amp; a.env_output[v] = s.er.output; a.env_holdcount[v] = s.er.holdcount; a.env_flags[v] = env_pack(s.er); }
+        voice_store<FILT, ENV>(a, v, s.phase, s.oout, s.fr, s.er);
         d.phase[v] = s.ph;
     }
 }
@@ -403,23 +378,6 @@ inline int launch_delay_one(const BankArgs& a, const DelayArgs& d, cudaStream_t 
     const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) { set_error("delay_bank_kernel launch: %s", cudaGetErrorString(e)); return MXB_ERR_CUDA; }
     return MXB_OK;
-}
-
-// outmode: DL_OUT_*; at least one of outmode / mix is set. MODK: the instantiations for blocks with a per-sample frequency / cutoff
-// (their own translation units, delay_km_*.cu)
-template <int FILT, bool MODK = false>
-inline int launch_delay_filt(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s) {
-#define MXB_D3(O, E)                                                                                 \
-    do {                                                                                             \
-        if (outmode == DL_OUT_F64)      return mix ? launch_delay_one<O, FILT, E, DL_OUT_F64, true, MODK>(a, d, s)   \
-                                                   : launch_delay_one<O, FILT, E, DL_OUT_F64, false, MODK>(a, d, s); \
-        else if (outmode == DL_OUT_F32) return mix ? launch_delay_one<O, FILT, E, DL_OUT_F32, true, MODK>(a, d, s)   \
-                                                   : launch_delay_one<O, FILT, E, DL_OUT_F32, false, MODK>(a, d, s); \
-        else                            return launch_delay_one<O, FILT, E, DL_OUT_NONE, true, MODK>(a, d, s);       \
-    } while (0)
-    if (osc_saw) { if (env) MXB_D3(OSC_T_SAW, 1); else MXB_D3(OSC_T_SAW, 0); }
-    else         { if (env) MXB_D3(OSC_T_GENERIC, 1); else MXB_D3(OSC_T_GENERIC, 0); }
-#undef MXB_D3
 }
 
 }  // namespace mxb

@@ -1,4 +1,4 @@
-// K2 interface: bank kernel with a maxiDelayline stage (see delay.cu).
+// K2 interface: bank kernel with a maxiDelayline stage (kernel: delay_impl.cuh; instantiations: delay_k.cu).
 #pragma once
 
 #include "bank_kernels.cuh"
@@ -33,25 +33,13 @@ struct DelayArgs {
     const double* size_tv;   // optional per-sample size argument [n_frames][V] (integral values), else NULL
 };
 
-// warps the K2 grid will have for V voices (the caller sizes the mix partials with it and passes it as a.W)
-int delay_bank_warps(int V);
+// warps the K2 grid will have for V voices: those that own at least one voice (the caller sizes the mix partials with it and
+// passes it as a.W)
+inline int delay_bank_warps(int V) { return (V + 31) / 32; }
 
-int launch_delay_bank(const BankArgs& a, const DelayArgs& d, int filt_kind, bool svf_lp, int env, bool out, bool mix,
-                      cudaStream_t s);
-
-// one launcher per filter family (delay_k_*.cu); outmode 0 none / 1 fp64 / 2 fp32
-int launch_delay_none(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_lores(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_hires(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_svf(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_svf_lp(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_biquad(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-// ... and for blocks with a per-sample oscillator frequency / filter cutoff (delay_km_*.cu)
-int launch_delay_none_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_lores_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_hires_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_svf_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_svf_lp_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
-int launch_delay_biquad_mod(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
+// The K2 instantiations of filter family FILT (FILT_T_*); MODK: those for blocks with a per-sample oscillator frequency / filter
+// cutoff. Defined in delay_k.cu, which build.py compiles once per family and MODK. outmode 0 none / 1 fp64 / 2 fp32.
+template <int FILT, bool MODK>
+int launch_delay_filt(const BankArgs& a, const DelayArgs& d, int osc_saw, int env, int outmode, bool mix, cudaStream_t s);
 
 }  // namespace mxb

@@ -57,21 +57,21 @@ K2_KEYS = [(f, o, e, om, mix, mk) for f in FILT_T for o in ("saw", "generic") fo
 
 def key_of(desc, call):
     """The instantiation a block runs: desc = dict(osc, filt, env, delay, svf_mix), call = dict(out, mix, f32, freq_tv, cutoff_tv)
-    (booleans). Restates the dispatch of mxb_bank_process_mod (bank.cu:543-570), launch_bank_filt (bank_kernels.cuh:469-489),
-    launch_delay_bank (delay.cu:8-31) and launch_delay_filt (delay_impl.cuh:410-423)."""
+    (booleans). Restates the dispatch of mxb_bank_process_mod (bank.cu:561-598), launch_bank_filt (bank_k.cu:11-41) and
+    launch_delay_filt (delay_k.cu:12-26)."""
     filt = desc["filt"]
     if filt == "svf" and tuple(float(x) for x in desc.get("svf_mix", (1.0, 0.0, 0.0, 0.0))) == (1.0, 0.0, 0.0, 0.0):
-        filt = "svf_lp"                                   # bank.cu:549-550: the SVF with mix (1, 0, 0, 0)
-    env = 1 if desc.get("env") else 0                     # bank.cu:547: ADSR and AR share ENV = 1 (env_ar is a runtime flag)
+        filt = "svf_lp"                                   # bank.cu:572-573: the SVF with mix (1, 0, 0, 0)
+    env = 1 if desc.get("env") else 0                     # bank.cu:565: ADSR and AR share ENV = 1 (env_ar is a runtime flag)
     fm, cm = bool(call.get("freq_tv")), bool(call.get("cutoff_tv"))
-    assert not (cm and filt not in CUTOFF_MOD), "per-sample cutoff is refused for this filter (bank.cu:482-484)"
+    assert not (cm and filt not in CUTOFF_MOD), "per-sample cutoff is refused for this filter (bank.cu:500-502)"
     if desc.get("delay"):
-        osc = "saw" if desc["osc"] == "saw" else "generic"                                 # delay.cu:9
-        outmode = "none" if not call["out"] else ("f32" if call["f32"] else "f64")      # delay.cu:10
-        mix = True if outmode == "none" else bool(call["mix"])                           # delay_impl.cuh:418: no output, bus only
-        return "k2", (filt, osc, env, outmode, mix, int(fm or cm))                       # delay.cu:11: any stream -> MODK
-    osc = {"sinewave": "sine", "phasor": "phasor", "saw": "saw"}.get(desc["osc"], "generic")    # bank.cu:543-546
-    return "k1", (filt, osc, env, bool(call["out"]), bool(call["mix"]), int(fm) | 2 * int(cm))  # bank_kernels.cuh:478-483
+        osc = "saw" if desc["osc"] == "saw" else "generic"                                 # bank.cu:584
+        outmode = "none" if not call["out"] else ("f32" if call["f32"] else "f64")      # bank.cu:585
+        mix = True if outmode == "none" else bool(call["mix"])                           # delay_k.cu:21: no output, bus only
+        return "k2", (filt, osc, env, outmode, mix, int(fm or cm))                       # bank.cu:586: any stream -> MODK
+    osc = {"sinewave": "sine", "phasor": "phasor", "saw": "saw"}.get(desc["osc"], "generic")    # bank.cu:561-564
+    return "k1", (filt, osc, env, bool(call["out"]), bool(call["mix"]), int(fm) | 2 * int(cm))  # bank_k.cu:24-29
 
 
 def kernel_key(symbol):
