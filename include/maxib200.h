@@ -461,6 +461,18 @@ typedef struct {
 int32_t mxb_stft_process3(mxb_stft* st, const float* in, int64_t stride_c, int64_t stride_t, int32_t n_samples,
                           int32_t max_frames, const mxb_stft_outputs* out, const mxb_stft_post* post, mxb_mfcc* mfcc,
                           int32_t* n_frames, int32_t mem, void* stream);
+/* Channels that advance independently, as separate maxiFFT objects do: channel c takes n_samples[c] >= 0 samples (host array [channels]),
+ * read at in[c*stride_c + t*stride_t], and fires frames_c = pos_c + n_samples[c] >= fft_size ? (pos_c + n_samples[c] - fft_size) / hop + 1
+ * : 0 frames, written to rows [c][0 .. frames_c) of the outputs of mxb_stft_process3 (same layouts, epilogues, MFCC and bars; the octave
+ * and Bark analysers at 1024 points only). n_frames: host array [channels], frames_c. In MXB_MEM_HOST mode rows frames_c .. of a channel
+ * up to the most frames any channel fired are overwritten with unspecified values. A negative count, frames_c > max_frames or more than
+ * 2^31 - 1 frames in all: MXB_ERR_INVALID, and the handle is unchanged.
+ * The handle keeps each channel's pos (maxiFFT::pos; mxb_stft_get_pos: host array [channels]). While they are all equal -- always, on a
+ * handle never driven ragged -- mxb_stft_process / 2 / 3 work as before; once they differ those calls return MXB_ERR_STATE. */
+int32_t mxb_stft_process_ragged(mxb_stft* st, const float* in, int64_t stride_c, int64_t stride_t, const int32_t* n_samples,
+                                int32_t max_frames, const mxb_stft_outputs* out, const mxb_stft_post* post, mxb_mfcc* mfcc,
+                                int32_t* n_frames, int32_t mem, void* stream);
+int32_t mxb_stft_get_pos(mxb_stft* st, int32_t* pos);
 /* maxiFFTOctaveAnalyzer::calculate(fftData) (src/libs/maxiFFT.cpp:261-300) on caller-supplied spectra, for every channel of o.
  * mags: float, frame f of channel c at ((c*max_frames)+f)*n_bands (the layout mxb_stft_process writes), frames 0..frames-1 analysed in
  * order. averages / peaks (each optional): float at ((c*max_frames)+f)*n_averages. The state is the handle's own: averages, peaks and
@@ -496,6 +508,12 @@ int32_t mxb_istft_create(mxb_ctx* ctx, int32_t channels, int32_t fft_size, int32
 int32_t mxb_istft_destroy(mxb_istft* st);
 int32_t mxb_istft_process(mxb_istft* st, const float* mags, const float* phases, int32_t frames, float* out,
                           int32_t mem, void* stream);
+/* Channels that advance independently: channel c resynthesises frames[c] frames (host array [channels], 0 .. max_frames), read at
+ * (c*max_frames + f)*bins of mags / phases, into out[c*max_frames*hop .. + frames[c]*hop). A channel with no frame keeps its overlap-add
+ * buffer. In MXB_MEM_HOST mode out samples past frames[c]*hop of a row, up to the most frames any channel has, are overwritten with
+ * unspecified values. A count outside 0 .. max_frames: MXB_ERR_INVALID, and the handle is unchanged. */
+int32_t mxb_istft_process_ragged(mxb_istft* st, const float* mags, const float* phases, const int32_t* frames, int32_t max_frames,
+                                 float* out, int32_t mem, void* stream);
 
 #ifdef __cplusplus
 }

@@ -913,7 +913,43 @@ public:
      * returns true on the sample that completes a frame); frames() tells how many per channel. maxFrames: rows per channel of the
      * result arrays (0 = enough for any nSamples). */
     bool process(const float* values, int nSamples, fftModes mode = WITH_POLAR_CONVERSION, int maxFrames = 0) {
+        return run(values, nSamples, nullptr, mode, maxFrames);
+    }
+    /* channels that advance independently, as separate maxiFFT objects do: channel c takes nSamples[c] samples (host array [channels]) of
+     * values, planar at a row pitch of the largest count, and fires its own frames; frames(c) tells how many. The attached analysers run
+     * on each channel's own frames: fused at fft size 1024; at other sizes the Bark analyser gets the fired frames packed, while the
+     * octave analyser (state per channel, advanced by whole calls of mxb_octave_process) needs every channel to fire as many frames as
+     * the others and throws MXB_ERR_UNSUPPORTED, before anything runs, when they would not. Returns true when any channel fired. */
+    bool process(const float* values, const int* nSamples, fftModes mode = WITH_POLAR_CONVERSION, int maxFrames = 0) {
+        if (!nSamples) throw maxiError(MXB_ERR_INVALID, "maxiFFT::process: nSamples is NULL");
+        return run(values, 0, nSamples, mode, maxFrames);
+    }
+    int frames() const { return frames_; }             /* the most frames any channel fired in the last call */
+    int frames(int channel) const { return framesC_.empty() ? 0 : framesC_[(size_t)channel]; }
+    int frameStride() const { return maxf_; }     /* frame f of channel c starts at ((c*frameStride()) + f)*getNumBins() */
+    std::vector<float>& getMagnitudes() { return mags_; }
+    std::vector<float>& getPhases() { return phases_; }
+    /* the spectral post-processors (src/libs/maxiFFT.cpp:101-132), computed by the same kernel while the magnitudes are on chip */
+    std::vector<float>& magsToDB() { return magsdb_; }                 /* laid out like getMagnitudes() */
+    std::vector<float>& getMagnitudesDB() { return magsdb_; }
+    std::vector<float>& spectralFlatness() { return flatness_; }       /* frame f of channel c at c*frameStride() + f */
+    std::vector<float>& spectralCentroid() { return centroid_; }
+    float* getReal() { return re_.data(); }
+    float* getImag() { return im_.data(); }
+    int getNumBins() { return bins_; }
+    int getFFTSize() { return fftSize_; }
+    int getHopSize() { return hop_; }
+    int getWindowSize() { return fftSize_; }
+private:
+    /* one block: every channel nSamples samples (counts NULL), or channel c counts[c] */
+    bool run(const float* values, int nSamples, const int* counts, fftModes mode, int maxFrames) {
         if (!h_) throw maxiError(MXB_ERR_STATE, "maxiFFT::process before setup()");
+        std::vector<int32_t> cnt, expect;
+        if (counts) {
+            cnt.assign(counts, counts + C_);
+            nSamples = 0;
+            for (int32_t k : cnt) nSamples = k > nSamples ? k : nSamples;           /* the row pitch */
+        }
         const int maxf = maxFrames > 0 ? maxFrames : nSamples / hop_ + 2;
         const size_t len = (size_t)C_ * (size_t)maxf * (size_t)bins_;
         const bool polar = mode == WITH_POLAR_CONVERSION;
@@ -955,67 +991,77 @@ public:
             }
         }
         const bool fused = post && fftSize_ == 1024;          /* the 1024-point kernel computes the analysers itself */
-        if (fused) {
+        if (counts && q.octave && !fused) {
+            /* the frames each channel will fire, from its position: mxb_octave_process advances every channel by the same count */
+            std::vector<int32_t> pos((size_t)C_);
+            maxib200_detail::check(mxb_stft_get_pos(h_, pos.data()), "mxb_stft_get_pos");
+            int first = -1;
+            for (int c = 0; c < C_; ++c) {
+                const long long a = (long long)pos[(size_t)c] + cnt[(size_t)c];
+                const int f = a >= fftSize_ ? (int)((a - fftSize_) / hop_) + 1 : 0;
+                if (c == 0) first = f;
+                else if (f != first)
+                    throw maxiError(MXB_ERR_UNSUPPORTED, "maxiFFT::process: an attached maxiFFTOctaveAnalyzer needs every channel to fire as many frames "
+                                                         "as the others at fft size " + std::to_string(fftSize_) + " (fused per channel at 1024 only)");
+            }
+        }
+        framesC_.assign((size_t)C_, 0);
+        if (counts) {
+            maxib200_detail::check(mxb_stft_process_ragged(h_, values, nSamples, 1, cnt.data(), maxf, &o, fused ? &q : nullptr, nullptr, framesC_.data(),
+                                                           MXB_MEM_HOST, nullptr), "mxb_stft_process_ragged");
+            for (int32_t f : framesC_) nf = f > nf ? f : nf;
+        } else if (fused) {
             maxib200_detail::check(mxb_stft_process3(h_, values, nSamples, 1, nSamples, maxf, &o, &q, nullptr, &nf, MXB_MEM_HOST, nullptr),
                                    "mxb_stft_process3");
         } else {
             maxib200_detail::check(mxb_stft_process2(h_, values, nSamples, 1, nSamples, maxf, &o, nullptr, &nf, MXB_MEM_HOST, nullptr),
                                    "mxb_stft_process2");
         }
+        if (!counts) framesC_.assign((size_t)C_, nf);
         if (post && !fused && nf > 0) {
-            /* frames 0 .. nf - 1 of every channel, in order */
+            /* frames 0 .. nf - 1 of every channel, in order (the same count for every channel: checked above) */
             if (q.octave)
                 maxib200_detail::check(mxb_octave_process(q.octave, mags_.data(), nf, maxf, q.octave_averages, q.octave_peaks, MXB_MEM_HOST, nullptr),
                                        "mxb_octave_process");
-            if (q.bark) runBark(nf, maxf);
+            if (q.bark) runBark(maxf);
         }
         frames_ = nf; maxf_ = maxf;
-        if (oct_ && oct_->h_ && nf > 0) { oct_->averages = const_cast<float*>(oct_->averagesOf(0, nf - 1)); oct_->peaks = const_cast<float*>(oct_->peaksOf(0, nf - 1)); }
-        if (bark_) bark_->last_ = nf > 0 ? nf - 1 : -1;
+        const int f0 = framesC_[0];
+        if (oct_ && oct_->h_ && f0 > 0) { oct_->averages = const_cast<float*>(oct_->averagesOf(0, f0 - 1)); oct_->peaks = const_cast<float*>(oct_->peaksOf(0, f0 - 1)); }
+        if (bark_) bark_->last_ = f0 > 0 ? f0 - 1 : -1;
         return nf > 0;
     }
-    int frames() const { return frames_; }
-    int frameStride() const { return maxf_; }     /* frame f of channel c starts at ((c*frameStride()) + f)*getNumBins() */
-    std::vector<float>& getMagnitudes() { return mags_; }
-    std::vector<float>& getPhases() { return phases_; }
-    /* the spectral post-processors (src/libs/maxiFFT.cpp:101-132), computed by the same kernel while the magnitudes are on chip */
-    std::vector<float>& magsToDB() { return magsdb_; }                 /* laid out like getMagnitudes() */
-    std::vector<float>& getMagnitudesDB() { return magsdb_; }
-    std::vector<float>& spectralFlatness() { return flatness_; }       /* frame f of channel c at c*frameStride() + f */
-    std::vector<float>& spectralCentroid() { return centroid_; }
-    float* getReal() { return re_.data(); }
-    float* getImag() { return im_.data(); }
-    int getNumBins() { return bins_; }
-    int getFFTSize() { return fftSize_; }
-    int getHopSize() { return hop_; }
-    int getWindowSize() { return fftSize_; }
-private:
-    /* Bark on the nf fired frames of every channel: in place when they are contiguous in the [C][maxf] layout, else packed into one
-     * call and the results put back at their rows */
-    void runBark(int nf, int maxf) {
+    /* Bark on the fired frames of every channel (frames(c) of channel c): in place when they are contiguous in the [C][maxf] layout, else
+     * packed into one call and the results put back at their rows */
+    void runBark(int maxf) {
         maxiBark& b = *bark_;
-        const size_t n = (size_t)C_ * (size_t)nf, bins = (size_t)bins_;
-        if (C_ == 1 || nf == maxf) {
+        size_t n = 0;
+        bool whole = true;
+        for (int c = 0; c < C_; ++c) { n += (size_t)framesC_[(size_t)c]; whole = whole && (framesC_[(size_t)c] == maxf || c == C_ - 1); }
+        const size_t bins = (size_t)bins_;
+        if (n == 0) return;
+        if (whole && (C_ == 1 || framesC_[0] == maxf)) {
             maxib200_detail::check(mxb_bark_process(b.handle(), mags_.data(), (int64_t)n, b.spec_.data(), b.rel_.data(), b.tot_.data(), MXB_MEM_HOST, nullptr),
                                    "mxb_bark_process");
             return;
         }
         b.rows_.resize(n * bins);
-        for (int c = 0; c < C_; ++c)
-            std::memcpy(&b.rows_[(size_t)c * nf * bins], &mags_[(size_t)c * maxf * bins], sizeof(float) * nf * bins);
+        for (size_t c = 0, k = 0; c < (size_t)C_; k += (size_t)framesC_[c], ++c)
+            std::memcpy(&b.rows_[k * bins], &mags_[c * maxf * bins], sizeof(float) * framesC_[c] * bins);
         std::vector<double> sp(n * 24), rl(n * 24), tt(n);
         maxib200_detail::check(mxb_bark_process(b.handle(), b.rows_.data(), (int64_t)n, sp.data(), rl.data(), tt.data(), MXB_MEM_HOST, nullptr),
                                "mxb_bark_process");
-        for (int c = 0; c < C_; ++c) {
-            const size_t src = (size_t)c * nf, dst = (size_t)c * maxf;
-            std::memcpy(&b.spec_[dst * 24], &sp[src * 24], sizeof(double) * 24 * nf);
-            std::memcpy(&b.rel_[dst * 24], &rl[src * 24], sizeof(double) * 24 * nf);
-            std::memcpy(&b.tot_[dst], &tt[src], sizeof(double) * nf);
+        for (size_t c = 0, k = 0; c < (size_t)C_; k += (size_t)framesC_[c], ++c) {
+            const size_t dst = c * (size_t)maxf, nfc = (size_t)framesC_[c];
+            std::memcpy(&b.spec_[dst * 24], &sp[k * 24], sizeof(double) * 24 * nfc);
+            std::memcpy(&b.rel_[dst * 24], &rl[k * 24], sizeof(double) * 24 * nfc);
+            std::memcpy(&b.tot_[dst], &tt[k], sizeof(double) * nfc);
         }
     }
     int C_, device_;
     mxb_ctx* ctx_ = nullptr; mxb_stft* h_ = nullptr;
     int fftSize_ = 0, hop_ = 0, bins_ = 0, frames_ = 0, maxf_ = 0;
+    std::vector<int32_t> framesC_;                          /* frames each channel fired in the last call */
     std::vector<float> mags_, phases_, re_, im_, magsdb_, flatness_, centroid_, hopbuf_;
     maxiFFTOctaveAnalyzer* oct_ = nullptr;
     maxiBark* bark_ = nullptr;
@@ -1081,6 +1127,19 @@ public:
     std::vector<float>& process(const std::vector<float>& data1, const std::vector<float>& data2, int frames, fftModes = SPECTRUM) {
         out_.resize((size_t)C_ * (size_t)frames * (size_t)hop_);
         maxib200_detail::check(mxb_istft_process(h_, data1.data(), data2.data(), frames, out_.data(), MXB_MEM_HOST, nullptr), "mxb_istft_process");
+        return out_;
+    }
+    /* channels that advance independently, as separate maxiIFFT objects do: channel c resynthesises frames[c] frames (host array
+     * [channels], 0 .. maxFrames) of data1 / data2, frame f of channel c at (c*maxFrames + f)*bins; returns planar [channels][maxFrames*hop],
+     * channel c's first frames[c]*hop samples its output. A channel with no frame keeps its overlap-add buffer. */
+    std::vector<float>& process(const std::vector<float>& data1, const std::vector<float>& data2, const int* frames, int maxFrames, fftModes = SPECTRUM) {
+        if (!frames) throw maxiError(MXB_ERR_INVALID, "maxiIFFT::process: frames is NULL");
+        const size_t need = (size_t)C_ * (size_t)(maxFrames > 0 ? maxFrames : 0) * (size_t)bins_;
+        if (data1.size() < need || data2.size() < need) throw maxiError(MXB_ERR_INVALID, "maxiIFFT::process: magnitudes / phases shorter than channels x maxFrames x numBins");
+        const std::vector<int32_t> fr(frames, frames + C_);
+        out_.assign((size_t)C_ * (size_t)(maxFrames > 0 ? maxFrames : 0) * (size_t)hop_, 0.f);
+        maxib200_detail::check(mxb_istft_process_ragged(h_, data1.data(), data2.data(), fr.data(), maxFrames, out_.data(), MXB_MEM_HOST, nullptr),
+                               "mxb_istft_process_ragged");
         return out_;
     }
     /* float process(mags, phases, mode), src/libs/maxiFFT.cpp:154-192 -- the reference's per-sample signature, for ONE channel: the spectrum is

@@ -35,6 +35,7 @@ EXPORTS = [
     "mxb_patch_get_ring", "mxb_patch_process", "mxb_patch_launch_count", "mxb_patch_set_mode", "mxb_patch_get_mode", "mxb_patch_codegen",
     "mxb_patch_create2", "mxb_patch_get_held", "mxb_patch_set_held",
     "mxb_octave_process", "mxb_bark_create", "mxb_bark_destroy", "mxb_bark_process",
+    "mxb_stft_process_ragged", "mxb_stft_get_pos", "mxb_istft_process_ragged",
 ]
 
 
@@ -142,6 +143,9 @@ def lib():
         "mxb_bark_create": (i32, [vp, i32, i32, pp]),
         "mxb_bark_destroy": (i32, [vp]),
         "mxb_bark_process": (i32, [vp, vp, i64, vp, vp, vp, i32, vp]),
+        "mxb_stft_process_ragged": (i32, [vp, vp, i64, i64, vp, i32, C.POINTER(StftOutputs), vp, vp, vp, i32, vp]),
+        "mxb_stft_get_pos": (i32, [vp, vp]),
+        "mxb_istft_process_ragged": (i32, [vp, vp, vp, vp, i32, vp, i32, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = the library does not export a declared symbol
@@ -464,6 +468,54 @@ class Stft:
                                      C.byref(nf), MEM_DEVICE, C.c_void_p(int(stream)) if stream else None), "mxb_stft_process")
         return nf.value
 
+    def positions(self):
+        """Each channel's maxiFFT::pos (mxb_stft_get_pos): int32 [C]."""
+        pos = np.zeros(self.C, dtype=np.int32)
+        check(lib().mxb_stft_get_pos(self.h, _np_ptr(pos)), "mxb_stft_get_pos")
+        return pos
+
+    def process_ragged(self, x, counts, want=("mags", "phases", "re", "im"), mfcc=None, octave=None, bark=False, features=False, max_frames=None):
+        """Channels that advance independently (mxb_stft_process_ragged): channel c takes counts[c] samples of x[c] (float32 [C][>= max
+        count] planar host array). Returns (frames int32 [C], dict of [C][max_frames][...] rows, channel c's first frames[c] of them
+        valid): 'mags' / 'phases' / 're' / 'im' ([bins]), 'mags_db' / 'flatness' / 'centroid' with features, 'mfcc' with an Mfcc,
+        'averages' / 'peaks' with an Octave, 'bark_specific' / 'bark_relative' / 'bark_total' with bark."""
+        x = np.ascontiguousarray(x, dtype=np.float32)
+        cnt = np.ascontiguousarray(counts, dtype=np.int32)
+        if x.ndim != 2 or x.shape[0] != self.C or cnt.shape != (self.C,):
+            raise MxbError(f"Stft.process_ragged: samples of shape {x.shape} and counts of shape {cnt.shape} for {self.C} channels")
+        maxf = int(max_frames) if max_frames is not None else max(1, (self.n + int(cnt.max(initial=0))) // self.hop + 1)
+        bins, C_ = self.bins, self.C
+        names = list(want) + (["mags_db", "flatness", "centroid"] if features else [])
+        r = {k: np.zeros((C_, maxf, bins) if k in ("mags", "phases", "re", "im", "mags_db") else (C_, maxf), dtype=np.float32) for k in names}
+        if mfcc is not None:
+            r["mfcc"] = np.zeros((C_, maxf, mfcc.coeffs))
+        o = StftOutputs(*[r[k].ctypes.data if k in r else None for k in ("mags", "phases", "re", "im", "mags_db", "flatness", "centroid", "mfcc")])
+        post = None
+        if octave is not None or bark:
+            if octave is not None:
+                r["averages"] = np.zeros((C_, maxf, octave.n_averages), dtype=np.float32); r["peaks"] = np.zeros_like(r["averages"])
+            if bark:
+                r["bark_specific"] = np.zeros((C_, maxf, 24)); r["bark_relative"] = np.zeros_like(r["bark_specific"]); r["bark_total"] = np.zeros((C_, maxf))
+            g = lambda k: r[k].ctypes.data if k in r else None
+            post = StftPost(octave.h if octave is not None else None, g("averages"), g("peaks"), 1 if bark else 0,
+                            g("bark_specific"), g("bark_relative"), g("bark_total"))
+        nf = np.zeros(C_, dtype=np.int32)
+        check(lib().mxb_stft_process_ragged(self.h, _np_ptr(x), x.shape[1], 1, _np_ptr(cnt), maxf, C.byref(o),
+                                            C.byref(post) if post is not None else None, mfcc.h if mfcc is not None else None,
+                                            _np_ptr(nf), MEM_HOST, None), "mxb_stft_process_ragged")
+        return nf, r
+
+    def process_ragged_device(self, in_ptr, stride_c, stride_t, counts, max_frames, mags=None, phases=None, re=None, im=None,
+                              mfcc=None, coeffs=None, stream=0):
+        """Device pointers (layouts of mxb_stft_process_ragged), asynchronous on `stream`; counts: host int array [C]. Returns frames [C]."""
+        cnt = np.ascontiguousarray(counts, dtype=np.int32)
+        o = StftOutputs(*[int(v) if v else None for v in (mags, phases, re, im, None, None, None, coeffs)])
+        nf = np.zeros(self.C, dtype=np.int32)
+        check(lib().mxb_stft_process_ragged(self.h, _ptr(in_ptr), stride_c, stride_t, _np_ptr(cnt), int(max_frames), C.byref(o), None,
+                                            mfcc.h if mfcc is not None else None, _np_ptr(nf), MEM_DEVICE,
+                                            C.c_void_p(int(stream)) if stream else None), "mxb_stft_process_ragged")
+        return nf
+
 
 class StftPost(C.Structure):
     _fields_ = [("octave", C.c_void_p), ("octave_averages", C.c_void_p), ("octave_peaks", C.c_void_p),
@@ -628,6 +680,26 @@ class Istft:
         out = np.empty((self.C, frames * self.hop), dtype=np.float32)
         check(lib().mxb_istft_process(self.h, _np_ptr(m), _np_ptr(p), frames, _np_ptr(out), MEM_HOST, None), "mxb_istft_process")
         return out
+
+    def process_ragged(self, mags, phases, frames):
+        """Channels that advance independently (mxb_istft_process_ragged): channel c resynthesises the first frames[c] of its rows of
+        float32 [C][max_frames][bins] mags / phases -> float32 [C][max_frames*hop], channel c's first frames[c]*hop samples valid."""
+        m = np.ascontiguousarray(mags, dtype=np.float32)
+        p = np.ascontiguousarray(phases, dtype=np.float32)
+        fr = np.ascontiguousarray(frames, dtype=np.int32)
+        if m.ndim != 3 or m.shape[0] != self.C or m.shape[2] != self.bins or p.shape != m.shape or fr.shape != (self.C,):
+            raise MxbError(f"Istft.process_ragged: spectra of shape {m.shape} / {p.shape}, frames {fr.shape}")
+        maxf = m.shape[1]
+        out = np.zeros((self.C, maxf * self.hop), dtype=np.float32)
+        check(lib().mxb_istft_process_ragged(self.h, _np_ptr(m), _np_ptr(p), _np_ptr(fr), maxf, _np_ptr(out), MEM_HOST, None),
+              "mxb_istft_process_ragged")
+        return out
+
+    def process_ragged_device(self, mags_ptr, phases_ptr, frames, max_frames, out_ptr, stream=0):
+        """Device pointers (layouts of mxb_istft_process_ragged), asynchronous on `stream`; frames: host int array [C]."""
+        fr = np.ascontiguousarray(frames, dtype=np.int32)
+        check(lib().mxb_istft_process_ragged(self.h, _ptr(mags_ptr), _ptr(phases_ptr), _np_ptr(fr), int(max_frames), _ptr(out_ptr), MEM_DEVICE,
+                                             C.c_void_p(int(stream)) if stream else None), "mxb_istft_process_ragged")
 
 
 # ------------------------------------------------------------------------------------------------ voice patches
